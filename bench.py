@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — cell-pairs/sec through the morpho_align EM loop (BASELINE.json metric) on B200.
+"""bench.py — cell-pairs/sec through the morpho_align EM loop (BASELINE.json metric) on an H100.
 
 Workload (default, = BASELINE configs[1]): one synthetic 3-D slice pair per GPU, 100,000 x 100,000 cells, 2,000 genes,
 KL dissimilarity, full EM (SVI_mode=False), K=15 inducing points, nn_init=True, max_iter=200. A *step* is one complete
@@ -17,12 +17,16 @@ KL dissimilarity, full EM (SVI_mode=False), K=15 inducing points, nn_init=True, 
                  MEASURED_PEAKS.json hbm_gbs; ``roofline_dense`` = the culling-off launches.
   cpu_baseline = the numpy oracle (port of the reference CPU path) on a bounded sample, host cores stated.
 
-``--impl reference`` times the reference's CPU algorithm (oracle port; the reference itself is pure Python and
-/root/reference does not exist on the GPU box) on a bounded sample: ONE EM iteration of a 20,000 x 20,000 pair per step
+``--impl reference`` times the reference's CPU algorithm (oracle port of the pure-Python reference) on a bounded sample: ONE EM iteration of a 20,000 x 20,000 pair per step
 (BASELINE.md section 4), W + K steps really executed; its ``config`` describes that sample.
 Other workloads: ``--workload vfc`` (BASELINE configs[4]), ``--workload chain`` (configs[2], multi-GPU slice chain).
 Multi-GPU (torchrun): one independent slice pair per rank (weak scaling) + ONE all-gather of the per-pair rigid
 transforms per step for the chain composition.
+
+``--dump-outputs DIR`` (pair workload): after the timed steps, the results of the last timed EM step as a caller of
+``Morpho_pairwise`` receives them (aligned coordinates, rigid transforms, scalars, column / row sums), one
+``DIR/<name>.npy`` each (float32 / float64, a few MB at the default size). The inputs are seeded, so two builds run with
+the same arguments can be compared output for output.
 """
 
 import argparse
@@ -67,7 +71,27 @@ def parse_args():
     ap.add_argument("--vfc-cells", type=int, default=1000000)
     ap.add_argument("--vfc-M", type=int, default=500)
     ap.add_argument("--vfc-iters", type=int, default=50)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (pair workload)")
+    args = ap.parse_args()
+    if args.dump_outputs is not None and (args.impl != "b200" or args.workload != "pair"):
+        ap.error("--dump-outputs is implemented for the default pair workload")
+    return args
+
+
+# results of Morpho_pairwise a caller reads after run(), in the caller's row order (P is not materialised in the timed path)
+DUMP_KEYS = ("XAHat", "RnA", "VnA", "optimal_RnA", "R", "t", "optimal_R", "optimal_t", "sigma2", "gamma", "sigma2_variance",
+             "K_NA", "K_NB")
+
+
+def dump_outputs(m, out_dir):
+    """Closes the solver's last EM run (D2H of the results, as ``run()`` does) and writes each result as <name>.npy."""
+    m._finish()
+    os.makedirs(out_dir, exist_ok=True)
+    for key in DUMP_KEYS:
+        a = np.asarray(getattr(m, key))
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        np.save(os.path.join(out_dir, f"{key}.npy"), a)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -110,7 +134,7 @@ def make_pair_on_device(n, G, dim, seed, device):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -259,7 +283,7 @@ def vfc_problem(n, M, D=3, seed=0):
 def run_vfc(args):
     """BASELINE configs[4]: SparseVFC on 1M 3-D cells, 500 control points, 50 EM iterations, 1 GPU. Metric: cell x
     control-point pairs per second through the public ``SparseVFC`` call (host arrays in / host arrays out, so the line's
-    ``value`` is end to end by construction). Roofline: the tcgen05 contraction of the normal equations, timed with CUDA
+    ``value`` is end to end by construction). Roofline: the wgmma contraction of the normal equations, timed with CUDA
     events inside the call (``timings``), against the measured dense bf16 tensor peak."""
     import torch
 
@@ -310,7 +334,7 @@ def run_vfc(args):
             peaks = json.load(f)
     except Exception:
         pass
-    peak_tf = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1650.0)))
+    peak_tf = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0)))
     tc_ms = float(np.mean([t["gram_tc_ms"].mean() for t in tms])) if "gram_tc_ms" in tms[0] else None
     flop = 2.0 * n * M * (M + D)  # SURVEY 8(d): 2 N M^2 + 2 N M D per iteration (the symmetric half would be N M^2)
     k_out = n // 10
@@ -322,10 +346,10 @@ def run_vfc(args):
         roofline = {
             "bound": "tensor", "kernel": "gram_tc_kernel (opt-in gram='tensor' arm)", "achieved": ach, "peak": peak_tf,
             "unit": "TFLOP/s", "frac": ach / peak_tf, "traffic": None,
-            "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (dense bf16)" if peaks else "fallback 1650 TFLOP/s",
+            "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained (dense bf16)" if peaks else "H100 SXM data sheet, 989 TFLOP/s dense bf16",
             "definition": "algorithmic FLOP of one launch (2 N M (M + D): U^T P U and U^T P Y of one EM iteration) / mean "
-                          "CUDA-event duration of spb_gram_tc (tcgen05 GEMM + 1% fp64 fold) inside the timed calls",
-            "note": "kind::tf32 peaks at half the bf16 rate and the fp32-accurate 3xTF32 split issues 3 MMAs per product: "
+                          "CUDA-event duration of spb_gram_tc (wgmma GEMM + 1% fp64 fold) inside the timed calls",
+            "note": "TF32 peaks at half the bf16 rate and the fp32-accurate 3xTF32 split issues 3 MMAs per product: "
                     "the ceiling of this formulation is peak / 6; the kernel re-reads its operands (A 128-row and B 256-row "
                     "panels per output tile, 8 B per element as hi/lo fp32), which makes it HBM-bound at this shape",
             "operand_bytes_per_launch": float((6 * 128 + 4 * 256 + 4 * 16) * 8.0 * n),
@@ -336,7 +360,7 @@ def run_vfc(args):
         "per_iteration_ms": {k: per_it(main["tms"], k) for k in ("estep_ms", "gram_ms", "solve_ms")},
         "gram_kernel": "weighted_gram_kernel (fp64 FMA, block upper triangle)",
         "gram_fp64_TFLOPs": float(n) * M * (M + 32) * 2 / (fp64_gram_ms * 1e-3) / 1e12,
-        "fp64_peak_TFLOPs_nominal": 37.0, "eigh_fallbacks": int(main["tms"][-1].get("eigh_fallbacks", 0)),
+        "fp64_peak_TFLOPs_nominal": 34.0, "eigh_fallbacks": int(main["tms"][-1].get("eigh_fallbacks", 0)),
     }
     tensor_arm = {
         "value": float(n) * M * (int(tens["out"]["iteration"]) + 1) / tens["sec"], "ms_per_step": tens["sec"] * 1e3,
@@ -775,6 +799,8 @@ def main():
                     launches=int(launches), clocks=clocks)
 
     main_arm = timed_arm(True, args.warmup, args.steps, True)
+    if args.dump_outputs is not None and rank == 0:
+        dump_outputs(m, args.dump_outputs)
     main_ev = timed_arm(True, 0, max(1, min(args.steps, 2)), False, events=True)   # per-launch sweep timings, same workload
     dense_arm = timed_arm(False, min(args.warmup, 1), max(1, min(args.steps, 2)), False)
     dense_ev = timed_arm(False, 0, 1, False, events=True)
@@ -790,7 +816,7 @@ def main():
             peaks = json.load(f)
     except Exception:
         pass
-    peak_gbs = float(peaks.get("hbm_gbs", 6650.0))
+    peak_gbs = float(peaks.get("hbm_gbs", 3350.0))
     nrb = m.ldx // _capi.ROW_TILE
     tiles_all = float(nrb) * cols
     # algorithmic bytes of one sweep launch = 4 B x (cell pairs the launch has to read): all pairs when dense, the visited
@@ -805,18 +831,9 @@ def main():
     dsw = dense_ev["sweeps"].reshape(-1, 2)
     d1, d2 = float(dsw[:, 0].mean()), float(dsw[:, 1].mean())
     alg_dense = 4.0 * NA * cols
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            tj = json.load(f)
-        if tj.get("cells") == args.cells and not args.svi:
-            traffic = tj.get(dom)
-    except Exception:
-        pass
     roofline = {
         "bound": "hbm", "kernel": dom, "achieved": dom_gbs, "peak": peak_gbs, "unit": "GB/s", "frac": dom_gbs / peak_gbs,
-        "peak_source": "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6650 GB/s",
-        "traffic": traffic,
+        "peak_source": "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s",
         "definition": "sum over the launches of 4 B x cell pairs the launch must read (visited tiles) / sum of CUDA-event "
                       "launch durations; the events are recorded in extra steps of the same workload right after the timed "
                       "ones, kernel by kernel (the timed steps replay whole iterations from CUDA graphs, which leaves no "

@@ -1,5 +1,5 @@
 /*
- * spateo_b200.h — C ABI of the B200-native morpho-align hot path (libspateo_b200.so).
+ * spateo_b200.h — C ABI of the H100-native (sm_90a) morpho-align hot path (libspateo_b200.so).
  *
  * The reference (aristoteleo/spateo-release @ 9ce1a90) is pure Python: it has NO FFI for this path. The seam a
  * maintainer would bind is the array-backend seam `check_backend()/nx.*` (spateo/alignment/methods/utils.py:35-66)
@@ -196,13 +196,13 @@ int spb_rows_normalize(const float* X, int64_t n, int64_t G, int64_t ldin, float
 int spb_gene_cost(const float* A, int64_t lda, const float* rowtermA, const float* B, int64_t ldb, const float* rowtermB,
                   int64_t NA, int64_t NB, int64_t G, int32_t metric, int32_t prob_type, float prob_param,
                   int32_t accumulate, float* GT, int64_t ldx, void* stream); /* utils.py:697,780-783,742 + :977-981 */
-/* tensor-core variant (tcgen05.mma kind::tf32, 3xTF32 split: operands given as hi/lo pairs, zero-padded to 32 features) */
+/* tensor-core variant (wgmma tf32, 3xTF32 split: operands given as hi/lo pairs, zero-padded to 32 features) */
 int spb_split_tf32(const float* x, float* hi, float* lo, int64_t n, void* stream);
 int spb_gene_cost_tc(const float* A_hi, const float* A_lo, int64_t lda, const float* rowtermA, const float* B_hi,
                      const float* B_lo, int64_t ldb, const float* rowtermB, int64_t NA, int64_t NB, int64_t G, int32_t metric,
                      int32_t prob_type, float prob_param, int32_t accumulate, float* GT, int64_t ldx,
                      void* stream); /* utils.py:697,780-783,742 + :977-981 */
-/* ---- K^T P K contraction on tcgen05 (3xTF32, fp32 accumulate per <= 4096-element slice, fp64 fold) ----------------------
+/* ---- K^T P K contraction on wgmma (3xTF32, fp32 accumulate per <= 4096-element slice, fp64 fold) ----------------------
    UtWU[k][l] = sum_n UT[k][n] w[n] UT[l][n]  (morpho_class.py:1266-1268; SparseVFC U^T P U, sparsevfc.py:189-198)
    UtX[k][e]  = sum_n UT[k][n] X[e][n], e < E <= 3  (morpho_class.py:1279)
    The tensor core's fp32 accumulator truncates, so the contraction runs on the row-centred kernel D = UT - mean (signed

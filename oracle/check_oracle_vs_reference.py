@@ -1,9 +1,9 @@
-"""TEST INFRASTRUCTURE ONLY — pins ``oracle/morpho_oracle.py`` against the unmodified reference (build container only).
+"""TEST INFRASTRUCTURE ONLY — pins ``oracle/morpho_oracle.py`` against the unmodified reference.
 
-Runs ``Morpho_pairwise`` from /root/reference and ``MorphoPairOracle`` on identical seeded inputs and prints the maximum
+Runs ``Morpho_pairwise`` from the reference checkout named by ``SPATEO_REFERENCE`` (oracle/ref_harness.py) and ``MorphoPairOracle`` on identical seeded inputs and prints the maximum
 deviation of every output. Expected: bitwise or ~1 ulp agreement (same numpy calls in the same order).
 
-    python oracle/check_oracle_vs_reference.py
+    SPATEO_REFERENCE=<spateo-release checkout> python oracle/check_oracle_vs_reference.py
 """
 
 import os

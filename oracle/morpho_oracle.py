@@ -10,9 +10,9 @@ executing the unmodified reference (``tests/golden/make_golden.py`` via ``oracle
 (``calc_distance``, ``get_P_core``, ``con_K``, ``inlier_from_NN``, ``voxel_data``) and end-to-end
 (``MorphoPairOracle.run`` vs ``Morpho_pairwise.run``: 2-D/3-D, SVI/full, float32/float64).
 Exception: ``sparse_vfc`` restates third-party ``dynamo-release>=1.4.1`` (``scVectorField.SparseVFC``), which is not in
-/root/reference and not installed: **parity unpinned** for that function (see its docstring).
+the reference tree and not installed: **parity unpinned** for that function (see its docstring).
 
-All ``file:line`` citations are relative to /root/reference/.
+All ``file:line`` citations are relative to the spateo-release tree.
 """
 
 from __future__ import annotations
@@ -858,7 +858,7 @@ def gp_velocity(X, vf, nonrigid_only=False):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# SparseVFC — PARITY UNPINNED (third-party dynamo-release>=1.4.1, not in /root/reference; SURVEY.md Appendix E)
+# SparseVFC — PARITY UNPINNED (third-party dynamo-release>=1.4.1, not in the reference tree; SURVEY.md Appendix E)
 # ---------------------------------------------------------------------------------------------------------------------
 
 

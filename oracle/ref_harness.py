@@ -1,6 +1,7 @@
-"""TEST INFRASTRUCTURE ONLY — imports the UNMODIFIED reference from /root/reference (SURVEY.md Appendix C).
+"""TEST INFRASTRUCTURE ONLY — imports the UNMODIFIED reference (SURVEY.md Appendix C) from the spateo-release checkout
+named by the environment variable ``SPATEO_REFERENCE``.
 
-Only usable in the build container (``/root/reference`` does not exist on the GPU box). It is used by
+Only usable where such a checkout exists; the test suite does not need it. It is used by
 ``tests/golden/make_golden.py`` to generate the committed golden fixtures and by ``oracle/check_oracle_vs_reference.py``
 to pin the numpy restatement in ``oracle/morpho_oracle.py`` against the real thing. Nothing in the product package,
 ``bench.py`` or the ``-m gpu`` tests imports this module.
@@ -15,11 +16,11 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("SPATEO_REFERENCE", "")
 
 
 def reference_available() -> bool:
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "spateo", "alignment", "methods"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "spateo", "alignment", "methods"))
 
 
 _loaded = {}
@@ -30,7 +31,7 @@ def load_reference():
     if "mc" in _loaded:
         return _loaded["mc"], _loaded["utils"]
     if not reference_available():
-        raise RuntimeError("reference tree not present (expected only in the build container)")
+        raise RuntimeError("reference tree not present: set SPATEO_REFERENCE to a spateo-release checkout")
     repo_root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     if repo_root not in sys.path:
         sys.path.insert(0, repo_root)

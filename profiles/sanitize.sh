@@ -1,8 +1,8 @@
 #!/bin/bash
 # compute-sanitizer over a small slice of the GPU parity suite (SURVEY.md section 5: race detection / sanitizers).
 # memcheck: out-of-bounds / misaligned accesses in every kernel the selected tests launch; racecheck: shared-memory hazards in
-# the streaming kernels (mbarrier-synchronised bulk-copy rings, tcgen05 kernels, the per-column radix select); synccheck:
-# barrier / mbarrier misuse. Usage (GPU box): bash profiles/sanitize.sh [memcheck|racecheck|synccheck|all]
+# the streaming kernels (mbarrier-synchronised bulk-copy rings, the TMA + wgmma kernels, the per-column radix select); synccheck:
+# barrier / mbarrier misuse. Usage (on an H100): bash profiles/sanitize.sh [memcheck|racecheck|synccheck|all]
 set -u
 TOOL=${1:-all}
 WIDE="(test_full_run_matches_reference and 2d_full]) or (test_sparse_estep_matches_float64_oracle and 0]) or (test_voxel_data_device_matches_host and 2-float32) or test_gene_cost_kl_matches_oracle or (test_kwargs_surface and large_K)"

@@ -1,4 +1,4 @@
-"""spateo_release_b200 — B200-native (sm_100a) implementation of Spateo's pairwise morpho-alignment hot path.
+"""spateo_release_b200 — H100-native (sm_90a) implementation of Spateo's pairwise morpho-alignment hot path.
 
 ``import spateo_release_b200 as st`` exposes the reference's namespaces for this path: ``st.align.morpho_align`` /
 ``Morpho_pairwise`` / ``BA_transform`` and ``st.tdr.morphofield_gp`` / ``morphofield_sparsevfc`` / ``morphofield``.

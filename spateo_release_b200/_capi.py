@@ -103,7 +103,7 @@ def load_library():
     if not os.path.exists(LIB_PATH):
         raise SpbError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). spateo_release_b200 has no CPU fallback."
+            "(nvcc, sm_90a). spateo_release_b200 has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)
     P, I32, I64, F, D = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_double
@@ -204,4 +204,4 @@ def require_cuda():
     import torch
 
     if not torch.cuda.is_available():
-        raise SpbError("spateo_release_b200 needs a CUDA device (sm_100a); there is no CPU fallback.")
+        raise SpbError("spateo_release_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback.")

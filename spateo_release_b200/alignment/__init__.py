@@ -1,4 +1,4 @@
-"""``st.align`` namespace of the B200-native hot path (reference: spateo/alignment/__init__.py:1-29)."""
+"""``st.align`` namespace of the H100-native hot path (reference: spateo/alignment/__init__.py:1-29)."""
 
 from .morpho_alignment import (
     compose_transformations,

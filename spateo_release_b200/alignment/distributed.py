@@ -8,6 +8,7 @@ exchange is ``[R(2x2) | t(2)]`` per pair (48 bytes), which is what BASELINE.json
 
 from __future__ import annotations
 
+import gc
 from typing import Callable, List, Optional
 
 import numpy as np
@@ -85,6 +86,23 @@ def morpho_align_chain_sharded(
     return models, transformation
 
 
+def pair_device_bytes(n_moving: int, n_fixed: int, n_genes: int) -> int:
+    """Device memory one prepared pair needs, dominated by its fp32 cost matrix [n_fixed][roundup(n_moving, 512)]; the
+    expression operands of the cost precompute (two sides, value + tf32 hi / lo, genes padded to 32) and 1 GiB for the
+    per-cell state are added on top."""
+    from .. import _capi
+
+    ldx = -(-n_moving // _capi.ROW_TILE) * _capi.ROW_TILE
+    gp = -(-n_genes // 32) * 32
+    return 4 * n_fixed * ldx + 4 * 3 * (n_moving + n_fixed) * gp + (1 << 30)
+
+
+def _room_for_next_pair(dev, need: int) -> bool:
+    """True when ``need`` bytes are free on ``dev``: driver-free memory plus what the caching allocator holds unused."""
+    free, _ = torch.cuda.mem_get_info(dev)
+    return free + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev) >= need
+
+
 def align_chain_pipelined(
     get_slice: Callable[[int], object],
     n_slices: int,
@@ -101,6 +119,10 @@ def align_chain_pipelined(
     overlaps them: the EM of pair p is only *enqueued* on the main stream (CUDA-graph replays, no host waits), and while it
     runs the host prepares pair p + world on a second stream — constructor, coarse initialisation, the staged host-to-device
     copy of its two expression matrices and its cost matrix — so that the next EM starts as soon as the current one ends.
+
+    The next pair is prepared early only when the device has room for its cost matrix beside the current pair's
+    (``pair_device_bytes``); otherwise the current pair is finished and freed first. Two 125k-cell cost matrices (63 GB each)
+    do not fit one 80 GB GPU, so such chains run one pair at a time.
 
     ``get_slice(k)`` returns slice k (AnnData-like, host arrays); only the slices of this rank's pairs are requested, and
     only they receive ``obsm[key_added]``. Returns ``(placed, transformations)`` with ``placed`` = {slice index: slice}.
@@ -129,6 +151,10 @@ def align_chain_pipelined(
         s.prepare()
         return s
 
+    def room_for(p):  # can pair p be prepared while the current pair still holds its buffers?
+        na, nb = slice_(p + 1).shape[0], slice_(p).shape[0]
+        return _room_for_next_pair(dev, pair_device_bytes(na, nb, slice_(p).shape[1]))
+
     local = {}
     t_pairs = []
     from .. import _capi
@@ -142,7 +168,7 @@ def align_chain_pipelined(
             cur = nxt
             cur.run_em()  # enqueued only: the host is free while the device iterates
             nxt = None
-            if i + 1 < len(mine):
+            if i + 1 < len(mine) and room_for(mine[i + 1]):
                 with torch.cuda.stream(side):
                     nxt = make(mine[i + 1])
             cur._finish()  # device -> host of the pair's results (waits for its EM)
@@ -151,6 +177,9 @@ def align_chain_pipelined(
             replayed += getattr(cur, "graph_replayed_launches", 0)
             del cur
             main.wait_stream(side)
+            if i + 1 < len(mine) and nxt is None:  # no room beside the current pair: prepare the next one in its place
+                gc.collect()  # the solver's buffers and captured graphs go back to the allocator before the next allocation
+                nxt = make(mine[i + 1])
             t_pairs.append(time.perf_counter() - t0)
     transformation = gather_transformations(local, n_pairs, device=dev if dist.is_initialized() and dist.get_backend() == "nccl" else None)
     placed = {}

@@ -1,5 +1,5 @@
 """``Morpho_pairwise`` — drop-in for ``spateo.alignment.methods.morpho_class.Morpho_pairwise`` (morpho_class.py:54)
-whose EM runs as hand-written sm_100a CUDA kernels behind the C ABI in ``include/spateo_b200.h``.
+whose EM runs as hand-written sm_90a CUDA kernels behind the C ABI in ``include/spateo_b200.h``.
 
 Host side (this file): validation, gene intersection, dense extraction, coordinate normalisation, inducing-point choice,
 coarse rigid initialisation bookkeeping and output wrapping — same names, argument meaning, RNG call order
@@ -60,9 +60,8 @@ _stage_lock = __import__("threading").Lock()
 
 def staged_to_device(host: np.ndarray, dev: torch.device) -> torch.Tensor:
     """Pageable host array -> device through two reusable pinned staging buffers (chunk k is copied into pinned memory
-    while chunk k-1 is on the wire): 36 GB/s measured for an 800 MB expression matrix against 11 GB/s for a pageable
-    ``.to()`` and a 0.6 s first-use cost for ``pin_memory()`` (profiles/h2d_micro.py). Counts the bytes in
-    ``TRANSFER_BYTES``."""
+    while chunk k-1 is on the wire), which avoids both a slow pageable ``.to()`` and the first-use cost of ``pin_memory()`` on
+    a large array. Counts the bytes in ``TRANSFER_BYTES``."""
     t = torch.from_numpy(np.ascontiguousarray(host, dtype=np.float32))
     _count_h2d(t)
     if t.is_pinned() or t.numel() < (2 << 20):
@@ -144,8 +143,8 @@ def resolve_device(device) -> torch.device:
 class GeneCostBuilder:
     """Device pipeline for ``calc_distance`` + ``calc_probability`` of one representation layer (utils.py:866-985).
 
-    Two contraction back-ends behind the same call: ``tensor`` (default) = tcgen05 / TMEM / TMA kernel with a 3xTF32
-    error-compensated split (fp32-accurate), ``simt`` = packed-FFMA2 register-tiled kernel with two-level accumulation.
+    Two contraction back-ends behind the same call: ``tensor`` (default) = wgmma / TMA kernel with a 3xTF32
+    error-compensated split (fp32-accurate), ``simt`` = register-tiled FFMA kernel with two-level accumulation.
     """
 
     def __init__(self, lib, dev, backend: Optional[str] = None):
@@ -899,12 +898,12 @@ class Morpho_pairwise:
                     cache[key] = t if t.is_pinned() else t.pin_memory()
 
     @staticmethod
-    def _choose_segments(nrb: int, nbb: int) -> int:
-        """Column segments so that CTAs ~ a multiple of the resident CTA slots (148 SMs x 2048 / ROW_TILE) and a segment is at most ``SPB_MAX_COLS_PER_CTA`` columns
+    def _choose_segments(nrb: int, nbb: int, n_sms: int) -> int:
+        """Column segments so that CTAs ~ a multiple of the resident CTA slots (n_sms x 2048 / ROW_TILE) and a segment is at most ``SPB_MAX_COLS_PER_CTA`` columns
         (short CTAs keep the tail of the last wave small once culling has shortened the column lists)."""
         cap = int(os.environ.get("SPB_MAX_COLS_PER_CTA", "4096"))
         max_seg = max(1, nbb // _capi.COL_STAGE)
-        slots = 148 * (2048 // _capi.ROW_TILE)  # resident CTAs of the sweeps on one B200
+        slots = n_sms * (2048 // _capi.ROW_TILE)  # resident CTAs of the sweeps
         seg = 1
         for waves in range(1, 256):
             seg = max(1, min(max_seg, (slots * waves) // max(nrb, 1)))
@@ -955,9 +954,10 @@ class Morpho_pairwise:
         s["colconst"] = torch.zeros((self._nbb_pad, _capi.CONST["SPB_COLCONST_FLOATS"]), dtype=f32, device=dev)
         s["colpart"] = torch.zeros((nrb, 4, self._nbb_pad), dtype=f32, device=dev)
         s["keepmask"] = torch.zeros((nrb, (self._nbb_pad + 31) // 32), dtype=torch.int32, device=dev)
-        seg1 = self._choose_segments(nrb, nbb)
-        seg2 = self._choose_segments(nrb, nbb)
-        seg_alloc = max(seg2, self._choose_segments(nrb, nbb_alloc))
+        n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        seg1 = self._choose_segments(nrb, nbb, n_sms)
+        seg2 = self._choose_segments(nrb, nbb, n_sms)
+        seg_alloc = max(seg2, self._choose_segments(nrb, nbb_alloc, n_sms))
         s["rowpart"] = torch.zeros((seg_alloc, 8, ldx), dtype=f32, device=dev)
         s["bbox"] = torch.zeros((nrb, 8), dtype=f32, device=dev)
         s["collist"] = torch.zeros((nrb, self._nbb_pad), dtype=torch.int32, device=dev)
@@ -1063,7 +1063,7 @@ class Morpho_pairwise:
         s["jacobi_ws"] = torch.zeros((1 + K * K,), dtype=f64, device=dev) if K <= _capi.MAX_K_FUSED else None
         p.jacobi_ws = None if s["jacobi_ws"] is None else s["jacobi_ws"].data_ptr()
         p.colmask = s["colmask"].data_ptr() if "colmask" in s else None
-        # K^T P K contraction: tcgen05 (3xTF32) above 32 inducing points, exact fp64 SIMT kernel for small K
+        # K^T P K contraction: wgmma (3xTF32) above 32 inducing points, exact fp64 SIMT kernel for small K
         backend = os.environ.get("SPB_GRAM", "auto")
         if backend == "tensor" or (backend == "auto" and K > 32):
             if "UT_hi" not in self.__dict__.setdefault("_gram", {}) or self._gram["UT_hi"].shape != self._UT.shape:
@@ -1442,7 +1442,8 @@ class Morpho_pairwise:
             # full (non-SVI) posterior with the final parameters (morpho_class.py:300-302)
             self.SVI_mode = False
             p.svi, p.NBb = 0, self.NB
-            p.seg1 = p.seg2 = self._choose_segments(self.ldx // _capi.ROW_TILE, self.NB)
+            p.seg1 = p.seg2 = self._choose_segments(self.ldx // _capi.ROW_TILE, self.NB,
+                                                    torch.cuda.get_device_properties(self._dev).multi_processor_count)
             self._NBb = self.NB
             self._estep_only(last_iter, st)
             # scalar Sp's must become the un-averaged sums (morpho_class.py:1183-1185)

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a kernels: bulk-async (TMA 1-D) copies, mbarriers, warp reductions,
+// Shared device helpers for the sm_90a kernels: bulk-async (TMA 1-D) copies, mbarriers, warp reductions,
 // digamma, small dense linear algebra in fp64.
 #pragma once
 #include <cuda_runtime.h>
@@ -19,6 +19,18 @@ static inline int spb_current_device() {
   int d = 0;
   cudaGetDevice(&d);
   return (d >= 0 && d < SPB_MAX_DEVICES) ? d : 0;
+}
+
+// SM count of the current device, for grid sizing (cached per device)
+static inline int spb_num_sms() {
+  static int n_dev[SPB_MAX_DEVICES] = {};
+  const int d = spb_current_device();
+  if (n_dev[d] == 0) {
+    int n = 0;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d);
+    n_dev[d] = n > 0 ? n : 1;
+  }
+  return n_dev[d];
 }
 
 #define SPB_CHECK_LAUNCH()                      \

@@ -6,15 +6,14 @@
 //   col_finalize   turns them into the per-column constants a_j, b_j, c_j (and K_NB_j).
 //   sweep 2  streams GT again and accumulates, per moving cell i (thread-owned registers), K_NA_spatial, K_NA_sigma2,
 //            sum_j Psigma d, K_NA and the D components of P @ XB.
-//   All pair arithmetic is packed fp32x2 (FADD2/FMUL2/FFMA2): the v1 scalar kernels were issue-bound at 22 instructions
-//   per cell pair (profiles/ncu_estep_r01_v1_summary.md).
+//   Pair arithmetic is written on fp32 pairs (two moving cells per value, explicitly rounded scalar operations).
 //   row_finalize   reduces the per-segment partials in fp64 and forms the global sums.
 //
 // Algorithmic HBM traffic: 4 bytes per cell pair per sweep (the fp32 g_ij), 8 B/pair/iteration in total.
 // Thread mapping: a CTA covers SPB_ROW_TILE = 512 moving cells: 128 consumer threads own 4 consecutive rows each (one
 // float4 of a GT row), one extra warp is the bulk-copy producer (160 threads, 96 registers, ~50 KB of shared memory:
-// 4 CTAs per SM). Column constants are broadcast from shared memory. 512-row tiles replaced the 1024-row tiles of
-// round 1: same dense speed, finer exact culling and shorter tails (profiles/launches_r02_full_summary.md).
+// 4 CTAs per SM). Column constants are broadcast from shared memory. 512-row tiles rather than 1024: finer exact culling
+// and shorter tails.
 #include "common.cuh"
 
 namespace {
@@ -85,7 +84,8 @@ __device__ __forceinline__ void producer_loop(SmemLayoutT<kColStage, kStages>& s
   }
 }
 
-// ---- packed fp32x2 arithmetic (Blackwell FADD2 / FMUL2 / FFMA2): two moving cells per instruction ------------------
+// ---- fp32 pairs: two moving cells per value. Hopper has no packed fp32x2 instructions, so every pair operation is two
+// scalar operations with explicit round-to-nearest (no contraction: the same bits as a packed add / mul / fma) ----------
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 pk(float a, float b) {
   u64 r;
@@ -94,24 +94,29 @@ __device__ __forceinline__ u64 pk(float a, float b) {
 }
 __device__ __forceinline__ void upk(u64 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
 __device__ __forceinline__ u64 add2(u64 a, u64 b) {
-  u64 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk(a, a0, a1);
+  upk(b, b0, b1);
+  return pk(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ u64 sub2(u64 a, u64 b) {
-  u64 r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk(a, a0, a1);
+  upk(b, b0, b1);
+  return pk(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
 }
 __device__ __forceinline__ u64 mul2(u64 a, u64 b) {
-  u64 r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk(a, a0, a1);
+  upk(b, b0, b1);
+  return pk(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
-  u64 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1;
+  upk(a, a0, a1);
+  upk(b, b0, b1);
+  upk(c, c0, c1);
+  return pk(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ u64 ex2_2(u64 v) {
   float a, b;
@@ -1318,7 +1323,7 @@ extern "C" int spb_posterior_argmax(const spb_em_params* p, int32_t iter, uint64
     cudaError_t e = cudaMemsetAsync(rowbest, 0, sizeof(uint64_t) * (size_t)p->NA, st);
     if (e != cudaSuccess) return (int)e;
     const int nrow = (p->NA + 255) / 256;
-    int nseg = (148 * 8 + nrow - 1) / nrow;
+    int nseg = (spb_num_sms() * 8 + nrow - 1) / nrow;  // ~8 CTAs per SM
     nseg = nseg < 1 ? 1 : (nseg > p->NBb ? p->NBb : nseg);
     row_argmax_kernel<<<dim3(nrow, nseg), 256, 0, st>>>(p->GT, p->ldx, batch_ptr(p, iter), p->colconst, p->XAHat, p->lm,
                                                         p->sc, p->NA, p->NBb, (unsigned long long*)rowbest);

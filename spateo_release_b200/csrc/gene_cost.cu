@@ -136,16 +136,20 @@ __device__ __forceinline__ u64 pk2(float a, float b) {
   return r;
 }
 __device__ __forceinline__ void upk2(u64 v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
+// Hopper has no packed fp32x2 instructions: each pair operation is two scalar round-to-nearest operations (same bits)
 __device__ __forceinline__ u64 add2p(u64 a, u64 b) {
-  u64 r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  return pk2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 constexpr int kFlush = 16;  // k-blocks (of 16 features) between folds of the register partial sums
 __device__ __forceinline__ u64 fma2p(u64 a, u64 b, u64 c) {
-  u64 r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  upk2(c, c0, c1);
+  return pk2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
 __global__ void __launch_bounds__(256, 2)
@@ -158,8 +162,8 @@ gene_cost_kernel(const float* __restrict__ A, int64_t lda, const float* __restri
   const int tx = t & 15, ty = t >> 4;
   const int64_t i0 = (int64_t)blockIdx.x * BM, j0 = (int64_t)blockIdx.y * BN;
   const int lrow = t >> 2, lq = t & 3;  // loader: rows lrow, lrow + 64; float4 quad lq
-  // 8 (fixed cells j) x 8 (moving cells i) micro-tile held as 8 x 4 packed fp32x2 accumulators: the inner product is
-  // FFMA2 with a scalar-broadcast j operand, i.e. half the issue slots of scalar FFMA
+  // 8 (fixed cells j) x 8 (moving cells i) micro-tile held as 8 x 4 fp32-pair accumulators; the inner product is an FFMA
+  // pair with a scalar-broadcast j operand
   u64 acc2[8][4];
 #pragma unroll
   for (int a = 0; a < 8; ++a)

@@ -1,94 +1,33 @@
-// Expression cost matrix on the 5th-generation tensor cores (tcgen05 + TMEM + TMA), fp32-accurate through a 3xTF32
-// split:  x = hi + lo  (hi = tf32(x), lo = x - hi),  A.B ~= Ahi.Bhi + Ahi.Blo + Alo.Bhi  accumulated in fp32 in TMEM.
+// Expression cost matrix on the Hopper tensor cores (wgmma + TMA + mbarrier), fp32-accurate through a 3xTF32 split:
+//   x = hi + lo  (hi = tf32(x), lo = x - hi),  A.B ~= Ahi.Bhi + Ahi.Blo + Alo.Bhi  accumulated in fp32 registers.
 // Same contract as gene_cost_kernel (gene_cost.cu): GT[j][i] (op)= prob(metric(A_i, B_j)).
 //
-// Per CTA (persistent, one per SM): tile = 128 fixed cells (UMMA M, TMEM lanes) x 256 moving cells (UMMA N, TMEM columns).
-//   warp 0   TMA producer: 2-stage ring, per k-block (32 features = one 128-byte swizzle row) four 2-D tensor-map loads
-//            (Bfix hi/lo 128x32, Amov hi/lo 256x32) into the canonical K-major SWIZZLE_128B layout
-//   warp 1   MMA issuer: 4 k-steps x 3 products of tcgen05.mma.kind::tf32 (M128 N256 K8) per k-block, tcgen05.commit
-//   warps 2-5 epilogue: tcgen05.ld (32 lanes x 32 columns), cost -> probability, store to GT; double-buffered TMEM
-//            accumulators (2 x 256 columns) so the epilogue of tile t overlaps the MMAs of tile t+1
-#include <cuda.h>
-
-#include "common.cuh"
+// Per CTA (persistent, one per SM): tile = 128 fixed cells (wgmma M, two warpgroups of 64) x 256 moving cells (wgmma N).
+//   warp 8      TMA producer: 2-stage ring, per k-block (32 features = one 128-byte swizzle row) four 2-D tensor-map loads
+//               (Bfix hi/lo 128x32, Amov hi/lo 256x32) into the canonical K-major SWIZZLE_128B layout
+//   warps 0-7   two consumer warpgroups, fixed cells 64 w .. 64 w + 63: 4 k-steps x 3 products of
+//               wgmma.m64n256k8.tf32 per k-block (128 fp32 accumulators per thread), then the epilogue
+//               (cost -> probability, store to GT) straight from the registers. The producer runs ahead into the next
+//               tile while the epilogue runs; the epilogue is a few per cent of a tile's MMA time at G ~ 2000.
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int TM = 128;   // fixed cells per tile (UMMA M)
-constexpr int TN = 256;   // moving cells per tile (UMMA N)
+constexpr int TM = 128;   // fixed cells per tile (2 x wgmma M)
+constexpr int TN = 256;   // moving cells per tile (wgmma N)
 constexpr int TK = 32;    // features per k-block (128 bytes)
 constexpr int kTcStages = 2;
-constexpr int kTcThreads = 192;  // 6 warps
+constexpr int kTcConsumers = 256;               // two warpgroups
+constexpr int kTcThreads = kTcConsumers + 32;   // + the producer warp
 
 struct __align__(1024) TcSmem {
   float bfix_hi[kTcStages][TM * TK];  // 16 KB each, SWIZZLE_128B K-major (8-row groups of 1024 B)
   float bfix_lo[kTcStages][TM * TK];
   float amov_hi[kTcStages][TN * TK];  // 32 KB each
   float amov_lo[kTcStages][TN * TK];
-  float rowterm_a[2][TN];             // per-tile row terms of the moving cells
   uint64_t full[kTcStages];
-  uint64_t empty[kTcStages];
-  uint64_t acc_full[2];
-  uint64_t acc_empty[2];
-  uint32_t tmem_base;
+  uint64_t empty[kTcStages];  // one arrive per consumer warpgroup
 };
-
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-               : "memory");
-}
-
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start address >> 4 in bits [0,14),
-// leading byte offset (unused for swizzled K-major, 1) in [16,30), stride byte offset = 1024 B (8 rows x 128 B) >> 4 in
-// [32,46), version 1 in [46,48), layout type SWIZZLE_128B = 2 in [61,64).
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(const void* smem) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_u32(smem) & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// cute::UMMA::InstrDescriptor for kind::tf32, fp32 accumulate, K-major A and B
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-  return (1u << 4)                    // c_format = F32
-         | (2u << 7)                  // a_format = TF32
-         | (2u << 10)                 // b_format = TF32
-         | ((uint32_t)(N >> 3) << 17) // n_dim
-         | ((uint32_t)(M >> 4) << 24);  // m_dim
-}
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "
-      "%25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]),
-        "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
 __device__ __forceinline__ float tc_cost_to_prob(float dot, float ta, float tb, int metric, int prob_type, float neg_inv2b) {
   float e;
@@ -104,8 +43,8 @@ __device__ __forceinline__ float tc_cost_to_prob(float dot, float ta, float tb, 
   return e;
 }
 
-// Tile order: bands of kBand fixed-cell tiles, moving-cell tiles fastest inside a band, so the ~148 tiles in flight
-// touch ~kBand B-side and ~148/kBand A-side operand panels (tens of MB, L2 resident) instead of 148 distinct A panels.
+// Tile order: bands of kBand fixed-cell tiles, moving-cell tiles fastest inside a band, so the tiles in flight (one
+// per SM) touch ~kBand B-side and ~SMs/kBand A-side operand panels (tens of MB, L2 resident) instead of one A panel each.
 constexpr int kBand = 16;
 __device__ __forceinline__ void tile_coords(int tile, int tiles_i, int tiles_j, int& ti, int& tj) {
   const int per_band = kBand * tiles_i;
@@ -130,25 +69,13 @@ gene_cost_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_c
   if (threadIdx.x == 0) {
     for (int s = 0; s < kTcStages; ++s) {
       mbar_init(&sm.full[s], 1);
-      mbar_init(&sm.empty[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&sm.acc_full[b], 1);
-      mbar_init(&sm.acc_empty[b], 4);  // one arrive per epilogue warp
+      mbar_init(&sm.empty[s], 2);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {  // TMEM allocation by one warp: all 512 columns (two 256-column accumulators)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)), "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = sm.tmem_base;
 
-  if (warp == 0) {
+  if (warp == kTcConsumers / 32) {
     // ===== TMA producer =====
     if (lane == 0) {
       int it = 0;
@@ -166,89 +93,72 @@ gene_cost_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one elected thread) =====
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_tf32(TM, TN);
-      int it = 0, t_local = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++t_local) {
-        const int buf = t_local & 1;
-        if (t_local >= 2) mbar_wait(&sm.acc_empty[buf], ((t_local >> 1) - 1) & 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(buf * TN);
-        for (int kb = 0; kb < nkb; ++kb, ++it) {
-          const int s = it % kTcStages;
-          mbar_wait(&sm.full[s], (it / kTcStages) & 1);
-          tc_fence_after();
-          const uint64_t d_bhi = umma_desc_k_sw128(sm.bfix_hi[s]), d_blo = umma_desc_k_sw128(sm.bfix_lo[s]);
-          const uint64_t d_ahi = umma_desc_k_sw128(sm.amov_hi[s]), d_alo = umma_desc_k_sw128(sm.amov_lo[s]);
-#pragma unroll
-          for (int k = 0; k < TK / 8; ++k) {
-            const uint64_t adv = (uint64_t)((k * 8 * 4) >> 4);  // 32 bytes per K = 8 step inside the 128-byte swizzle row
-            // UMMA "A" (M side) = fixed cells, "B" (N side) = moving cells; small cross terms first
-            umma_tf32(tmem_d, d_blo + adv, d_ahi + adv, idesc, (kb | k) != 0);
-            umma_tf32(tmem_d, d_bhi + adv, d_alo + adv, idesc, 1);
-            umma_tf32(tmem_d, d_bhi + adv, d_ahi + adv, idesc, 1);
-          }
-          umma_commit(&sm.empty[s]);  // frees the smem stage once these MMAs have read it
-        }
-        umma_commit(&sm.acc_full[buf]);  // accumulator complete -> epilogue
-      }
-    }
-  } else {
-    // ===== epilogue warps (2..5): TMEM lanes 32 * (warp % 4) =====
-    const int q = warp & 3;
-    const int et = threadIdx.x - 64;  // 0..127
-    int t_local = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++t_local) {
-      const int buf = t_local & 1;
-      int ti, tj;
-      tile_coords(tile, tiles_i, tiles_j, ti, tj);
-      const int64_t j = (int64_t)tj * TM + q * 32 + lane;
-      const int64_t i0 = (int64_t)ti * TN;
-      // stage the moving cells' row terms of this tile
-      for (int c = et; c < TN; c += 128) sm.rowterm_a[buf][c] = (rtA != nullptr && i0 + c < NA) ? rtA[i0 + c] : 0.f;
-      named_bar_sync(2, 128);
-      const float tb = (rtB != nullptr && j < NB) ? rtB[j] : 0.f;
-      mbar_wait(&sm.acc_full[buf], (t_local >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * TN);
-#pragma unroll 1
-      for (int c0 = 0; c0 < TN; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld32(taddr + (uint32_t)c0, r);
-        if (j < NB) {
-          float* dst = GT + j * ldx + i0 + c0;
-#pragma unroll
-          for (int c = 0; c < 32; c += 4) {
-            if (i0 + c0 + c < ldx) {
-              float o[4];
-#pragma unroll
-              for (int u = 0; u < 4; ++u) {
-                const int64_t i = i0 + c0 + c + u;
-                o[u] = i < NA ? tc_cost_to_prob(__uint_as_float(r[c + u]), sm.rowterm_a[buf][c0 + c + u], tb, metric,
-                                                prob_type, neg_inv2b)
-                              : 0.f;
-              }
-              float4* d4 = reinterpret_cast<float4*>(dst + c);
-              if (accumulate) {
-                const float4 old = *d4;
-                o[0] *= old.x; o[1] *= old.y; o[2] *= old.z; o[3] *= old.w;
-              }
-              *d4 = make_float4(o[0], o[1], o[2], o[3]);
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.acc_empty[buf]);
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+
+  // ===== consumer warpgroups: wgmma "A" (M side) = fixed cells, "B" (N side) = moving cells =====
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int row0 = wg * 64 + (t >> 5) * 16 + (lane >> 2);  // this thread's rows row0, row0 + 8 of the tile
+  const int col0 = 2 * (lane & 3);                           // and columns 8 n + col0 + {0, 1}
+  const uint32_t a_off = (uint32_t)(wg * 64 * TK * 4);       // this warpgroup's 64 fixed-cell rows (8 KB, 1024-aligned)
+  float acc[TN / 2];
+  int it = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    int ti, tj;
+    tile_coords(tile, tiles_i, tiles_j, ti, tj);
+#pragma unroll
+    for (int c = 0; c < TN / 2; ++c) acc[c] = 0.f;
+    for (int kb = 0; kb < nkb; ++kb, ++it) {
+      const int s = it % kTcStages;
+      mbar_wait(&sm.full[s], (it / kTcStages) & 1);
+      const uint64_t d_bhi = wgmma_desc_k_sw128((const uint8_t*)sm.bfix_hi[s] + a_off);
+      const uint64_t d_blo = wgmma_desc_k_sw128((const uint8_t*)sm.bfix_lo[s] + a_off);
+      const uint64_t d_ahi = wgmma_desc_k_sw128(sm.amov_hi[s]), d_alo = wgmma_desc_k_sw128(sm.amov_lo[s]);
+      wgmma_fence_operand(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TK / 8; ++k) {
+        const uint64_t adv = (uint64_t)((k * 8 * 4) >> 4);  // 32 bytes per K = 8 step inside the 128-byte swizzle row
+        wgmma_tf32_m64n256k8(acc, d_blo + adv, d_ahi + adv, 1);  // small cross terms first
+        wgmma_tf32_m64n256k8(acc, d_bhi + adv, d_alo + adv, 1);
+        wgmma_tf32_m64n256k8(acc, d_bhi + adv, d_ahi + adv, 1);
+      }
+      wgmma_commit();
+      // the previous k-block's MMAs are done reading their stage: hand it back to the producer
+      wgmma_wait<1>();
+      wgmma_fence_operand(acc);
+      if (kb > 0 && t == 0) mbar_arrive(&sm.empty[(it - 1) % kTcStages]);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operand(acc);
+    if (t == 0) mbar_arrive(&sm.empty[(it - 1) % kTcStages]);
+
+    const int64_t i0 = (int64_t)ti * TN;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t j = (int64_t)tj * TM + row0 + 8 * h;
+      if (j >= NB) continue;
+      const float tb = rtB != nullptr ? rtB[j] : 0.f;
+      float* dst = GT + j * ldx + i0 + col0;
+#pragma unroll
+      for (int n = 0; n < TN / 8; ++n) {  // fully unrolled: acc must stay in registers
+        const int64_t i = i0 + 8 * n + col0;
+        if (i >= ldx) continue;  // ldx % 4 == 0 and i even: i + 1 < ldx as well
+        float o[2];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const float ta = (rtA != nullptr && i + u < NA) ? rtA[i + u] : 0.f;
+          o[u] = i + u < NA ? tc_cost_to_prob(acc[4 * n + 2 * h + u], ta, tb, metric, prob_type, neg_inv2b) : 0.f;
+        }
+        float2* d2 = reinterpret_cast<float2*>(dst + 8 * n);
+        if (accumulate) {
+          const float2 old = *d2;
+          o[0] *= old.x;
+          o[1] *= old.y;
+        }
+        *d2 = make_float2(o[0], o[1]);
+      }
+    }
   }
 }
 

@@ -1,37 +1,36 @@
-// K^T P K contraction on the 5th-generation tensor cores (tcgen05 + TMEM + TMA):
+// K^T P K contraction on the Hopper tensor cores (wgmma + TMA + mbarrier):
 //     UtWU[k][l] = sum_n U[n][k] w[n] U[n][l]          (morpho_class.py:1266-1268  U^T diag(K_NA) U;  SparseVFC U^T P U)
 //     UtX[k][e]  = sum_n U[n][k] X[n][e]               (morpho_class.py:1279       U^T PXB_term;      SparseVFC U^T P Y)
 // as ONE K-major GEMM  C = A B^T, fp32-accurate through the 3xTF32 split  x = hi + lo,
-// a b ~= a_hi b_hi + a_hi b_lo + a_lo b_hi  accumulated in fp32 in TMEM.
+// a b ~= a_hi b_hi + a_hi b_lo + a_lo b_hi  accumulated in fp32 registers.
 //
-// The tensor core's fp32 accumulator TRUNCATES, which biases a sum of all-positive terms (U > 0, w >= 0) by ~4e-6
-// relative (measured); so the contraction runs on the CENTRED kernel  D = U - 1 m^T  (m_k = mean_n U[n][k]):
+// The tensor core's fp32 accumulation TRUNCATES, which biases a sum of all-positive terms (U > 0, w >= 0) by ~4e-6
+// relative; so the contraction runs on the CENTRED kernel  D = U - 1 m^T  (m_k = mean_n U[n][k]):
 //     A = D^T  [K][N]                       (constant over the EM: gram_center_kernel, once)
 //     B = [ w o D^T ; X^T ; w^T ]  [K + E + 1][N]   (rebuilt every iteration by gram_prepare_kernel)
 //     UtWU = D^T W D + m v^T + v m^T + (sum w) m m^T,   v = D^T w  (the extra B row),   UtX = D^T X + m (sum_n X)^T
 // whose terms change sign, so the truncation errors cancel instead of adding up (same idea as the centred KL contraction
 // of gene_cost_tc.cu). The rank-one corrections are applied in fp64 by gram_reduce_kernel.
 //
-// Work unit = (output tile 128 x <=256, slice of the reduction dimension n). Every unit flushes its fp32 TMEM accumulator
+// Work unit = (output tile 128 x <=256, slice of the reduction dimension n). Every unit flushes its fp32 accumulators
 // to a scratch slab; gram_reduce_kernel folds the slices in fp64 in a fixed order (deterministic), symmetrises the K x K
 // block and writes the fp64 outputs the solve kernels consume. Slices are short (<= kMaxSliceKb k-blocks) so the fp32
 // accumulation inside the tensor core never runs over more than a few thousand terms.
 //
-//   warp 0    TMA producer: 2-stage ring; per k-block (32 reduction elements = one 128-byte swizzle row) the A tile
-//             (128 rows, hi and lo) and the B tile (128 or 256 rows, hi and lo) as 2-D tensor-map boxes of 128 rows
-//   warp 1    MMA issuer: 4 k-steps x 3 products of tcgen05.mma.kind::tf32 (M128, N = 16..256, K8) per k-block
-//   warps 2-5 epilogue: tcgen05.ld (32 lanes x 32 columns) -> scratch slab
-#include <cuda.h>
-
-#include "common.cuh"
+//   warp 8     TMA producer: 2-stage ring; per k-block (32 reduction elements = one 128-byte swizzle row) the A tile
+//              (128 rows, hi and lo) and the B tile (128 or 256 rows, hi and lo) as 2-D tensor-map boxes of 128 rows
+//   warps 0-7  two consumer warpgroups (A rows 64 w .. 64 w + 63): 4 k-steps x 3 products of wgmma.m64nNk8.tf32 per
+//              k-block, N = 128 or 256 (the tile's columns rounded up), then the accumulators -> scratch slab
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int GM = 128;  // output rows per tile (UMMA M, TMEM lanes)
-constexpr int GN = 256;  // output columns per tile (UMMA N, TMEM columns)
+constexpr int GM = 128;  // output rows per tile (2 x wgmma M)
+constexpr int GN = 256;  // output columns per tile (largest wgmma N)
 constexpr int GK = 32;   // reduction elements per k-block (128 bytes)
 constexpr int kGStages = 2;
-constexpr int kGThreads = 192;
+constexpr int kGConsumers = 256;             // two warpgroups
+constexpr int kGThreads = kGConsumers + 32;  // + the producer warp
 constexpr int kMaxTiles = 16;     // (K + E) <= 515 -> at most 5 x 3 tiles, upper block triangle + right-hand sides
 constexpr int kMaxSliceKb = 128;  // k-blocks per unit: fp32 accumulation over at most 4096 reduction elements
 
@@ -41,9 +40,7 @@ struct __align__(1024) GramSmem {
   float b_hi[kGStages][GN * GK];  // 32 KB each (two stacked 128-row boxes)
   float b_lo[kGStages][GN * GK];
   uint64_t full[kGStages];
-  uint64_t empty[kGStages];
-  uint64_t acc_full;
-  uint32_t tmem_base;
+  uint64_t empty[kGStages];  // one arrive per consumer warpgroup
 };
 
 struct GramPlan {
@@ -53,54 +50,53 @@ struct GramPlan {
   int nkb;              // k-blocks in total
   int K, E;
   int8_t mt[kMaxTiles], nt[kMaxTiles];
-  int16_t ncols[kMaxTiles];     // UMMA N of the tile (multiple of 16)
+  int16_t ncols[kMaxTiles];     // columns of the tile (multiple of 16)
   int8_t index[8][4];           // (mt, nt) -> tile slot or -1
 };
 
-__device__ __forceinline__ void g_tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
-               : "memory");
+template <int N>
+__device__ __forceinline__ void gram_wgmma(float (&acc)[N / 2], uint64_t a, uint64_t b) {
+  if constexpr (N == 256) wgmma_tf32_m64n256k8(acc, a, b, 1);
+  else wgmma_tf32_m64n128k8(acc, a, b, 1);
 }
-// K-major SWIZZLE_128B shared-memory matrix descriptor (see gene_cost_tc.cu)
-__device__ __forceinline__ uint64_t g_desc_k_sw128(const void* smem) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_u32(smem) & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__device__ __forceinline__ uint32_t g_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void g_umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void g_umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void g_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void g_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void g_tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "
-      "%25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]),
-        "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+
+// Consumer warpgroup of one unit with an N-column accumulator: MMAs over the unit's k-blocks, then the scratch slab.
+template <int N>
+__device__ __forceinline__ void gram_consume(GramSmem& sm, int kb0, int kb1, float* __restrict__ scratch) {
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, lane = threadIdx.x & 31;
+  const uint32_t a_off = (uint32_t)(wg * 64 * GK * 4);  // this warpgroup's 64 A rows (8 KB, 1024-aligned)
+  float acc[N / 2];
+#pragma unroll
+  for (int c = 0; c < N / 2; ++c) acc[c] = 0.f;
+  for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
+    const int s = it % kGStages;
+    mbar_wait(&sm.full[s], (it / kGStages) & 1);
+    const uint64_t d_ahi = wgmma_desc_k_sw128((const uint8_t*)sm.a_hi[s] + a_off);
+    const uint64_t d_alo = wgmma_desc_k_sw128((const uint8_t*)sm.a_lo[s] + a_off);
+    const uint64_t d_bhi = wgmma_desc_k_sw128(sm.b_hi[s]), d_blo = wgmma_desc_k_sw128(sm.b_lo[s]);
+    wgmma_fence_operand(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < GK / 8; ++k) {
+      const uint64_t adv = (uint64_t)((k * 8 * 4) >> 4);
+      gram_wgmma<N>(acc, d_alo + adv, d_bhi + adv);  // small cross terms first
+      gram_wgmma<N>(acc, d_ahi + adv, d_blo + adv);
+      gram_wgmma<N>(acc, d_ahi + adv, d_bhi + adv);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's stage is no longer read: hand it back to the producer
+    wgmma_fence_operand(acc);
+    if (it > 0 && t == 0) mbar_arrive(&sm.empty[(it - 1) % kGStages]);
+  }
+  wgmma_wait<0>();
+  wgmma_fence_operand(acc);
+  const int row = wg * 64 + (t >> 5) * 16 + (lane >> 2), col = 2 * (lane & 3);
+  float* dst = scratch + ((int64_t)blockIdx.x * GM + row) * GN + col;
+#pragma unroll
+  for (int n = 0; n < N / 8; ++n) {
+    *reinterpret_cast<float2*>(dst + 8 * n) = make_float2(acc[4 * n], acc[4 * n + 1]);
+    *reinterpret_cast<float2*>(dst + 8 * GN + 8 * n) = make_float2(acc[4 * n + 2], acc[4 * n + 3]);
+  }
 }
 
 // One CTA = one work unit (tile, slice).
@@ -114,81 +110,38 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_consta
   const int tile = blockIdx.x % plan.ntiles, slice = blockIdx.x / plan.ntiles;
   const int mt = plan.mt[tile], nt = plan.nt[tile], ncols = plan.ncols[tile];
   const int kb0 = slice * plan.kb_per_slice, kb1 = min(plan.nkb, kb0 + plan.kb_per_slice);
-  const int nb_boxes = (ncols + 127) / 128;  // 128-row boxes of the B operand
+  // 128-row boxes of the B operand = wgmma N / 128. A tile narrower than 128 columns (e.g. the right-hand sides alone, E + 1
+  // columns) still runs N = 128 on zero-filled rows: its MMAs are a small share of the contraction, and gram_reduce_kernel
+  // reads only the tile's ncols columns.
+  const int nb_boxes = ncols > 128 ? 2 : 1;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kGStages; ++s) {
       mbar_init(&sm.full[s], 1);
-      mbar_init(&sm.empty[s], 1);
+      mbar_init(&sm.empty[s], 2);
     }
-    mbar_init(&sm.acc_full, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)), "r"(GN)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  g_fence_before();
   __syncthreads();
-  g_fence_after();
-  const uint32_t tmem_base = sm.tmem_base;
 
-  if (warp == 0) {
+  if (warp == kGConsumers / 32) {
     if (lane == 0) {
       for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
         const int s = it % kGStages;
         if (it >= kGStages) mbar_wait(&sm.empty[s], ((it / kGStages) - 1) & 1);
         mbar_expect_tx(&sm.full[s], (uint32_t)((2 * GM + 2 * 128 * nb_boxes) * GK * 4));
-        g_tma_load_2d(sm.a_hi[s], &map_a_hi, kb * GK, mt * GM, &sm.full[s]);
-        g_tma_load_2d(sm.a_lo[s], &map_a_lo, kb * GK, mt * GM, &sm.full[s]);
+        tma_load_2d(sm.a_hi[s], &map_a_hi, kb * GK, mt * GM, &sm.full[s]);
+        tma_load_2d(sm.a_lo[s], &map_a_lo, kb * GK, mt * GM, &sm.full[s]);
         for (int b = 0; b < nb_boxes; ++b) {
-          g_tma_load_2d(sm.b_hi[s] + b * 128 * GK, &map_b_hi, kb * GK, nt * GN + b * 128, &sm.full[s]);
-          g_tma_load_2d(sm.b_lo[s] + b * 128 * GK, &map_b_lo, kb * GK, nt * GN + b * 128, &sm.full[s]);
+          tma_load_2d(sm.b_hi[s] + b * 128 * GK, &map_b_hi, kb * GK, nt * GN + b * 128, &sm.full[s]);
+          tma_load_2d(sm.b_lo[s] + b * 128 * GK, &map_b_lo, kb * GK, nt * GN + b * 128, &sm.full[s]);
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = g_idesc_tf32(GM, ncols);
-      for (int kb = kb0, it = 0; kb < kb1; ++kb, ++it) {
-        const int s = it % kGStages;
-        mbar_wait(&sm.full[s], (it / kGStages) & 1);
-        g_fence_after();
-        const uint64_t d_ahi = g_desc_k_sw128(sm.a_hi[s]), d_alo = g_desc_k_sw128(sm.a_lo[s]);
-        const uint64_t d_bhi = g_desc_k_sw128(sm.b_hi[s]), d_blo = g_desc_k_sw128(sm.b_lo[s]);
-#pragma unroll
-        for (int k = 0; k < GK / 8; ++k) {
-          const uint64_t adv = (uint64_t)((k * 8 * 4) >> 4);
-          g_umma_tf32(tmem_base, d_alo + adv, d_bhi + adv, idesc, (it | k) != 0);  // small cross terms first
-          g_umma_tf32(tmem_base, d_ahi + adv, d_blo + adv, idesc, 1);
-          g_umma_tf32(tmem_base, d_ahi + adv, d_bhi + adv, idesc, 1);
-        }
-        g_umma_commit(&sm.empty[s]);
-      }
-      g_umma_commit(&sm.acc_full);
-    }
-  } else {
-    const int q = warp & 3;  // TMEM lane quarter owned by this warp
-    mbar_wait(&sm.acc_full, 0);
-    g_fence_after();
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-    float* dst = scratch + ((int64_t)blockIdx.x * GM + q * 32 + lane) * GN;
-    for (int c0 = 0; c0 < ncols; c0 += 32) {
-      uint32_t r[32];
-      g_tmem_ld32(taddr + (uint32_t)c0, r);
-#pragma unroll
-      for (int c = 0; c < 32; c += 4)
-        *reinterpret_cast<float4*>(dst + c0 + c) = make_float4(__uint_as_float(r[c]), __uint_as_float(r[c + 1]),
-                                                                __uint_as_float(r[c + 2]), __uint_as_float(r[c + 3]));
-    }
-    g_fence_before();
+    return;
   }
-  g_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(GN) : "memory");
-  }
+  if (nb_boxes == 2) gram_consume<256>(sm, kb0, kb1, scratch);
+  else gram_consume<128>(sm, kb0, kb1, scratch);
 }
 
 // fp64 fold of the slice partials in slice order; K x K block symmetrised over the tiles that were computed.
@@ -377,7 +330,7 @@ int make_plan(int K, int E, int64_t N, GramPlan* plan) {
       ++p.ntiles;
     }
   p.nkb = (int)((N + GK - 1) / GK);
-  int want = (2 * 148 + p.ntiles - 1) / p.ntiles;  // slices for ~2 units per SM
+  int want = (2 * spb_num_sms() + p.ntiles - 1) / p.ntiles;  // slices for ~2 units per SM
   int per = (p.nkb + want - 1) / want;
   if (per < 8) per = 8;
   if (per > kMaxSliceKb) per = kMaxSliceKb;
@@ -415,7 +368,8 @@ extern "C" int spb_gram_prepare(const float* UT, int64_t ldn, int64_t N, int32_t
   int gx = (int)((N / 4 + 255) / 256);
   if (gx > 592) gx = 592;
   if (gx < 1) gx = 1;
-  if ((int64_t)gx * (K + E + 1) > 148 * 64) gx = (148 * 64) / (K + E + 1) + 1;  // enough CTAs, short rows need no more
+  const int n_sm = spb_num_sms();
+  if ((int64_t)gx * (K + E + 1) > n_sm * 64) gx = (n_sm * 64) / (K + E + 1) + 1;  // enough CTAs, short rows need no more
   gram_prepare_kernel<<<dim3(gx, K + E + 1), 256, 0, ST>>>(UT, ldn, N, K, E, mean, w, X, ldxx, B_hi, B_lo, sums4);
   SPB_CHECK_LAUNCH();
   return 0;

@@ -88,7 +88,7 @@ constexpr int kGT = 64;        // tile edge
 constexpr int kGC = 32;        // rows of n per shared-memory chunk
 constexpr int kAccRows = 128;  // granularity of the row chunks
 inline int gram_rows_per_block(int64_t N, int npairs) {
-  const int64_t want_chunks = (2 * 148 + npairs - 1) / npairs;
+  const int64_t want_chunks = (2 * spb_num_sms() + npairs - 1) / npairs;  // ~2 CTAs per SM
   int64_t rows = (N + want_chunks - 1) / want_chunks;
   rows = ((rows + kAccRows - 1) / kAccRows) * kAccRows;
   if (rows < 2 * kAccRows) rows = 2 * kAccRows;
@@ -810,7 +810,7 @@ extern "C" int spb_update_gamma_alpha(const spb_em_params* p, void* stream) {
 extern "C" int spb_nonrigid_accumulate(const spb_em_params* p, void* stream) {
   pxb_term_kernel<<<(p->NA + 255) / 256, 256, 0, ST>>>(*p);
   SPB_CHECK_LAUNCH();
-  if (p->UT_hi != nullptr) {  // tensor-core contraction (tcgen05, 3xTF32): every K the caller prepared operands for
+  if (p->UT_hi != nullptr) {  // tensor-core contraction (wgmma, 3xTF32): every K the caller prepared operands for
     int rc = spb_gram_prepare(p->UT, p->ldx, p->NA, p->K, p->UT_mean, p->K_NA, p->PXB_term, p->ldx, 3, p->GB_hi, p->GB_lo,
                               p->gram_sums, stream);
     if (rc) return rc;

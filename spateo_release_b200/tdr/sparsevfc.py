@@ -77,7 +77,7 @@ def SparseVFC(
     ``timings`` are extras).
 
     ``gram``: how the normal-equation blocks U^T P U and U^T P Y are contracted — ``"fp64"`` (= ``"auto"``, the default) =
-    SIMT kernels with fp64 products, the reference-accurate path; ``"tensor"`` (opt-in) = tcgen05 kernel (3xTF32 on the
+    SIMT kernels with fp64 products, the reference-accurate path; ``"tensor"`` (opt-in) = wgmma kernel (3xTF32 on the
     row-centred kernel matrix, fp64 fold). The tensor path's products carry fp32-level relative noise (~1e-7), which is the
     relative size of SparseVFC's own regulariser lambda sigma2 K against U^T P U at the default lambda: it therefore solves with
     a ridge just above that noise floor and returns a slightly SMOOTHER fit than the reference solution (7x faster at
@@ -227,7 +227,7 @@ def SparseVFC(
             t = np.array([[e[0].elapsed_time(e[1]), e[1].elapsed_time(e[2]), e[2].elapsed_time(e[3])] for e in ev_pairs])
             timings.update(estep_ms=t[:, 0], gram_ms=t[:, 1], solve_ms=t[:, 2], gram="tensor" if use_tc else "fp64",
                            eigh_fallbacks=n_fallback)
-            if use_tc:  # split of gram_ms: operand preparation | tcgen05 contraction + fp64 fold
+            if use_tc:  # split of gram_ms: operand preparation | tensor-core contraction + fp64 fold
                 timings["gram_prepare_ms"] = np.array([e[1].elapsed_time(e[4]) for e in ev_pairs])
                 timings["gram_tc_ms"] = np.array([e[4].elapsed_time(e[2]) for e in ev_pairs])
         C = Cd[:, :D].cpu().numpy()

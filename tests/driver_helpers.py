@@ -31,7 +31,7 @@ def driver_chain(n_slices=4, g=24, seed=7):
 
 
 def models_from_golden(g, n_slices=4):
-    """The same chain rebuilt from the fixture (the GPU box has no RNG-order dependence on this helper)."""
+    """The same chain rebuilt from the fixture (no RNG-order dependence on this helper)."""
     import pandas as pd
 
     from spateo_release_b200.anndata_lite import AnnDataLite

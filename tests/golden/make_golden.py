@@ -1,4 +1,4 @@
-"""Generate the golden fixtures in this directory by EXECUTING THE UNMODIFIED REFERENCE (build container only).
+"""Generate the golden fixtures in this directory by EXECUTING THE UNMODIFIED REFERENCE (needs SPATEO_REFERENCE).
 
     python tests/golden/make_golden.py
 

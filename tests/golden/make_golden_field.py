@@ -1,6 +1,6 @@
 """Generate tests/golden/case_field_geometry.npz by running the UNMODIFIED reference's GPVectorField functions
 (spateo/tdr/morphometrics/morphofield_dg/GPVectorField.py, morphofield/gaussian_process.py) on seeded synthetic
-fields. Build-container only (needs /root/reference):  python tests/golden/make_golden_field.py
+fields. Needs the reference:  SPATEO_REFERENCE=<spateo-release checkout> python tests/golden/make_golden_field.py
 """
 
 import io

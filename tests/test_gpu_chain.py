@@ -119,6 +119,27 @@ def test_pipelined_chain_equals_serial_chain():
     assert np.allclose(placed[0].obsm["align_spatial"], models[0].obsm["spatial"])
 
 
+def test_pipelined_chain_without_room_for_two_pairs(monkeypatch):
+    """When the device cannot hold the next pair beside the current one (two 125k-cell cost matrices on an 80 GB GPU),
+    align_chain_pipelined frees the current pair before preparing the next: same transformations as the serial driver."""
+    import spateo_release_b200 as st
+    from spateo_release_b200.alignment import distributed
+
+    asked = []
+    monkeypatch.setattr(distributed, "_room_for_next_pair", lambda dev, need: asked.append(need) or False)
+    models, _ = _chain(n_slices=4, n=2200)
+    kw = dict(verbose=False, SVI_mode=False, max_iter=80)
+    np.random.seed(0)
+    tr_serial = st.align.morpho_align_transformation([m.copy() for m in models], device="0", **kw)
+    np.random.seed(0)
+    mine = [m.copy() for m in models]
+    placed, tr = st.align.align_chain_pipelined(lambda k: mine[k], 4, device="0", **kw)
+    assert len(asked) == 2 and all(n > 4 * 2200 * 2200 for n in asked)
+    for a, b in zip(tr_serial, tr):
+        assert np.allclose(a["Rotation"], b["Rotation"], atol=1e-5) and np.allclose(a["Translation"], b["Translation"], atol=1e-3)
+    assert sorted(placed) == [0, 1, 2, 3]
+
+
 def test_gather_transformations_under_nccl_resolves_index_strings():
     """With an NCCL process group the slab must live on the CUDA device even when the package-style device string ("0") or
     None is passed (round-1 advisor finding); single rank, so no second GPU is needed."""

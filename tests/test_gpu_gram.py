@@ -1,6 +1,6 @@
 """GPU: the K^T P K contraction kernels (morpho_class.py:1266-1279; SparseVFC normal equations) against float64 numpy.
 
-``spb_gram_tc`` = tcgen05 / TMEM / TMA kernel with the 3xTF32 split on the row-centred kernel (fp32-accurate products, fp32
+``spb_gram_tc`` = wgmma / TMA kernel with the 3xTF32 split on the row-centred kernel (fp32-accurate products, fp32
 accumulation over at most 4096 reduction elements, fp64 fold and rank-one corrections); ``spb_weighted_gram`` = fp64 SIMT kernels (small-K variant below 33 inducing points).
 """
 

@@ -560,7 +560,7 @@ def test_inlier_from_NN_device_matches_oracle(D):
 
 KW_VARIANTS = {
     "large_K_eigh_path": dict(K=80, max_iter=100),
-    # the K^T P K contraction runs on tcgen05 above 32 inducing points; 64 = largest in-library Jacobi, 200 / 500 = cuSOLVER
+    # the K^T P K contraction runs on the tensor cores above 32 inducing points; 64 = largest in-library Jacobi, 200 / 500 = cuSOLVER
     # eigen-solve with the factorised field apply
     "K64_tensor_gram": dict(K=64, max_iter=100),
     "K200_tensor_gram": dict(K=200, max_iter=100),

@@ -54,7 +54,7 @@ def test_sparsevfc_matches_oracle(D, n, M, gram="fp64"):
 
 
 def test_sparsevfc_tensor_path_is_a_regularised_fit():
-    """``gram="tensor"`` (opt-in): the tcgen05 contraction delivers the normal equations with fp32-level relative noise
+    """``gram="tensor"`` (opt-in): the tensor-core contraction delivers the normal equations with fp32-level relative noise
     (~1e-7). SparseVFC's own regulariser lambda sigma2 K sits at that same relative level of U^T P U, so the tensor path has
     to add a ridge above its noise floor and is therefore a slightly smoother fit, NOT the reference solution: it must
     recover the same inliers / noise level / smooth field, and its distance to the fp64 path is printed."""

@@ -162,12 +162,12 @@ def test_argmax_key_decoding_and_transpose():
 def test_segment_choice_respects_the_column_cap(monkeypatch):
     from spateo_release_b200.alignment.morpho_class import Morpho_pairwise
 
-    seg = Morpho_pairwise._choose_segments(98, 100000)
+    seg = Morpho_pairwise._choose_segments(98, 100000, 132)  # H100 SXM
     assert (100000 + seg - 1) // seg <= 4096 and seg * 98 >= 296
     monkeypatch.setenv("SPB_MAX_COLS_PER_CTA", "1024")
-    seg2 = Morpho_pairwise._choose_segments(98, 100000)
+    seg2 = Morpho_pairwise._choose_segments(98, 100000, 132)
     assert seg2 > seg and (100000 + seg2 - 1) // seg2 <= 1024
-    assert Morpho_pairwise._choose_segments(1, 240) >= 1
+    assert Morpho_pairwise._choose_segments(1, 240, 132) >= 1
 
 
 def test_svc_field_descriptor_and_oracle_jacobian():
@@ -241,3 +241,26 @@ def test_graph_unroll_choice():
     assert f(SimpleNamespace(graph_unroll=0, SVI_mode=True, NA=100000, NB=100000, batch_size=10000)) == 8
     assert f(SimpleNamespace(graph_unroll=0, SVI_mode=False, NA=5000, NB=5000, batch_size=None)) == 8
     assert f(SimpleNamespace(graph_unroll=3, SVI_mode=False, NA=100000, NB=100000, batch_size=None)) == 3
+
+
+def test_two_125k_cost_matrices_do_not_fit_80_gb():
+    """The prefetch estimate of the chain driver: one 125k-cell pair fits an 80 GB H100, two do not."""
+    from spateo_release_b200.alignment.distributed import pair_device_bytes
+
+    one = pair_device_bytes(125000, 125000, 2000)
+    assert 4 * 125000 * 125440 < one < 80e9 < 2 * one
+
+
+def test_library_built_with_other_nvcc_flags_is_rebuilt(tmp_path, monkeypatch):
+    """A library with no record of its nvcc flags, or built for another target (say sm_100a), is stale."""
+    import __graft_entry__ as ge
+
+    lib, stamp = tmp_path / "lib.so", tmp_path / "lib.so.flags"
+    lib.write_bytes(b"")
+    monkeypatch.setattr(ge, "LIB", str(lib))
+    monkeypatch.setattr(ge, "FLAGS_STAMP", str(stamp))
+    assert ge._stale()
+    stamp.write_text(" ".join(ge.NVCC_FLAGS).replace("sm_90a", "sm_100a"))
+    assert ge._stale()
+    stamp.write_text(" ".join(ge.NVCC_FLAGS))
+    assert not ge._stale()

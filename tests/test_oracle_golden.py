@@ -1,7 +1,8 @@
 """CPU: pins oracle/morpho_oracle.py against golden vectors produced by executing the unmodified reference
-(tests/golden/make_golden.py). Bitwise in the build container; tolerances below allow for a different host BLAS."""
+(tests/golden/make_golden.py). Bitwise with the host BLAS they were made with; tolerances below allow for a different one."""
 
 import ast
+import contextlib
 
 import numpy as np
 import pytest
@@ -84,13 +85,28 @@ def test_preparation_matches_reference(golden, case):
         assert np.array_equal(orc.batch_perm, g["pre_batch_perm"])
 
 
+GOLDEN_BLAS_THREADS = 8  # OpenBLAS threads of the reference runs that made the fixtures
+
+
+def golden_blas_threads():
+    """A threaded BLAS sums in an order that depends on its thread count, and 100+ EM iterations carry that difference
+    past the float64 tolerance: run with the thread count the fixtures were made with, whatever the host's core count.
+    Without threadpoolctl the BLAS keeps its own thread count."""
+    try:
+        from threadpoolctl import threadpool_limits
+    except ImportError:
+        return contextlib.nullcontext()
+    return threadpool_limits(limits=GOLDEN_BLAS_THREADS, user_api="blas")
+
+
 @pytest.mark.parametrize("case", CASES)
 @pytest.mark.parametrize("dtype", ["float32", "float64"])
 def test_full_run_matches_reference(golden, case, dtype):
     g = golden(case)
     sfx = "" if dtype == "float32" else "_f64"
     orc = _make_oracle(g, dtype)
-    orc.run()
+    with golden_blas_threads():
+        orc.run()
     scale = np.abs(g["final_optimal_RnA" + sfx]).max()
     tol = 2e-4 if dtype == "float32" else 1e-6
     for key in ("optimal_RnA", "XAHat", "RnA"):
@@ -104,6 +120,29 @@ def test_full_run_matches_reference(golden, case, dtype):
             assert (P > 0).sum(0).max() <= cfg_sparse(g)  # at most top_k stored entries per column
         num = np.linalg.norm(P.astype(np.float64) - g["final_P" + sfx])
         assert num / np.linalg.norm(g["final_P" + sfx]) < (2e-2 if dtype == "float32" else 1e-5)
+
+
+@pytest.mark.parametrize("case", ["2d_full", "3d_svi_sparse32"])
+@pytest.mark.parametrize("dtype", ["float32", "float64"])
+def test_oracle_is_bitwise_equal_to_the_reference(golden, case, dtype):
+    """Every final output the reference run stored (posterior or its row / column sums, aligned coordinates, Coff, R, t,
+    the closing similarity, sigma2, gamma) is reproduced by the oracle to the last bit: same numpy calls in the same order,
+    with the BLAS thread count the fixtures were made with."""
+    pytest.importorskip("threadpoolctl", reason="pinning the BLAS thread count needs threadpoolctl")
+    g = golden(case)
+    sfx = "" if dtype == "float32" else "_f64"
+    orc = _make_oracle(g, dtype)
+    with golden_blas_threads():
+        orc.run()
+    # sparse mode stores only the row / column sums, taken like the fixture did (on the sparse matrix)
+    derived = {"P_rowsum": np.asarray(orc.P.sum(1)).reshape(-1), "P_colsum": np.asarray(orc.P.sum(0)).reshape(-1),
+               "P": orc.P.toarray() if hasattr(orc.P, "toarray") else orc.P}
+    keys = [k[len("final_"):len(k) - len(sfx)] for k in g if k.startswith("final_") and k.endswith(sfx)
+            and (sfx or not k.endswith("_f64"))]
+    assert {"Coff", "R", "t", "optimal_t", "XAHat", "optimal_RnA"} <= set(keys)
+    for key in keys:
+        got = derived[key] if key in derived else getattr(orc, key)
+        assert np.array_equal(np.asarray(got, dtype=np.float64), np.asarray(g[f"final_{key}{sfx}"], dtype=np.float64)), key
 
 
 def test_ba_transform_reproduces_training_points(golden):
