@@ -147,7 +147,7 @@ typedef struct spb_em_params {
   double* Coff;                /* [K][3] */
   double* moments;             /* [32] rigid-update moment accumulator */
   double* jacobi_ws;           /* [1 + K*K] eigenbasis of the previous non-rigid solve ([0] = K once valid): Jacobi warm start, or NULL */
-  const float* UT_hi;          /* [K][ldx] tf32 split of the row-centred UT (tensor-core K^T P K contraction), or NULL = SIMT path */
+  const float* UT_hi;          /* [K][ldx] tf32 split of the row-centred UT (tensor-core K^T P K contraction); required when K > 32, NULL selects the fp64 kernel for K <= 32 */
   const float* UT_lo;          /* [K][ldx] */
   const float* UT_mean;        /* [K] row means of UT (spb_gram_center) */
   float* GB_hi;                /* [K+4][ldx] per-iteration B operand [K_NA o D ; PXB_term^T ; K_NA], hi part */
@@ -192,11 +192,8 @@ int spb_kl_prepare_rows(const float* X, int64_t n, int64_t G, int64_t ldin, floa
 /* row squared norms (euc) or row-normalisation (cos) */
 int spb_rows_sqnorm(const float* X, int64_t n, int64_t G, int64_t ldin, float* rowterm, void* stream); /* utils.py:780 */
 int spb_rows_normalize(const float* X, int64_t n, int64_t G, int64_t ldin, float* out, int64_t ldout, void* stream); /* utils.py:736-739 */
-/* GT[j][i] (op)= prob(metric(A_i, B_j)); A:[NA][G] pitch lda, B:[NB][G] pitch ldb; accumulate!=0 multiplies into GT */
-int spb_gene_cost(const float* A, int64_t lda, const float* rowtermA, const float* B, int64_t ldb, const float* rowtermB,
-                  int64_t NA, int64_t NB, int64_t G, int32_t metric, int32_t prob_type, float prob_param,
-                  int32_t accumulate, float* GT, int64_t ldx, void* stream); /* utils.py:697,780-783,742 + :977-981 */
-/* tensor-core variant (wgmma tf32, 3xTF32 split: operands given as hi/lo pairs, zero-padded to 32 features) */
+/* GT[j][i] (op)= prob(metric(A_i, B_j)); A:[NA][G] pitch lda, B:[NB][G] pitch ldb; accumulate!=0 multiplies into GT.
+   wgmma tf32 with a 3xTF32 split: each operand is given as the hi/lo pair of spb_split_tf32, zero-padded to 32 features */
 int spb_split_tf32(const float* x, float* hi, float* lo, int64_t n, void* stream);
 int spb_gene_cost_tc(const float* A_hi, const float* A_lo, int64_t lda, const float* rowtermA, const float* B_hi,
                      const float* B_lo, int64_t ldb, const float* rowtermB, int64_t NA, int64_t NB, int64_t G, int32_t metric,
@@ -224,8 +221,6 @@ int spb_label_cost(const int32_t* labA, const int32_t* labB, const float* LT, in
                    int32_t accumulate, float* GT, int64_t ldx, void* stream); /* utils.py:830 */
 
 /* ---- E-step: calc_distance(euc) + get_P_core + row/col sums, P never materialised ---------------------------- */
-/* diagnostics of the two sweep kernels: cfg = 16 * mode, mode 0 = product, 1 = stream only, 2 = arithmetic only (profiles/sweep_micro.py) */
-int spb_set_sweep_config(int32_t cfg);
 int spb_gather_cols(const spb_em_params* p, int32_t iter, void* stream);   /* morpho_class.py:1149 */
 /* row-block bounding boxes + per-block column work lists (exact zero-tile culling when p->cull) — new, no reference line */
 int spb_estep_col_lists(const spb_em_params* p, void* stream);

@@ -11,7 +11,6 @@ stays on the device, there is no host synchronisation inside the iteration loop 
 from __future__ import annotations
 
 import ctypes as C
-import os
 from typing import List, Optional, Union
 
 import numpy as np
@@ -91,24 +90,6 @@ def _round_up(x: int, m: int) -> int:
     return ((x + m - 1) // m) * m
 
 
-class _nvtx:
-    """NVTX range (``SPB_NVTX=1``) around the phases of an alignment, for nsys / ncu --nvtx timelines."""
-
-    enabled = os.environ.get("SPB_NVTX", "0") == "1"
-
-    def __init__(self, name: str):
-        self.name = name
-
-    def __enter__(self):
-        if self.enabled:
-            torch.cuda.nvtx.range_push(self.name)
-
-    def __exit__(self, *exc):
-        if self.enabled:
-            torch.cuda.nvtx.range_pop()
-        return False
-
-
 def morton_order(coords: np.ndarray) -> np.ndarray:
     """Row permutation that sorts points along a Z-order curve (isotropic quantisation: 16 bits/axis in 2-D, 10 in 3-D)."""
     c = np.asarray(coords, dtype=np.float64)
@@ -143,15 +124,11 @@ def resolve_device(device) -> torch.device:
 class GeneCostBuilder:
     """Device pipeline for ``calc_distance`` + ``calc_probability`` of one representation layer (utils.py:866-985).
 
-    Two contraction back-ends behind the same call: ``tensor`` (default) = wgmma / TMA kernel with a 3xTF32
-    error-compensated split (fp32-accurate), ``simt`` = register-tiled FFMA kernel with two-level accumulation.
+    The contraction is a wgmma / TMA kernel with a 3xTF32 error-compensated split (fp32-accurate).
     """
 
-    def __init__(self, lib, dev, backend: Optional[str] = None):
-        import os
-
+    def __init__(self, lib, dev):
         self.lib, self.dev = lib, dev
-        self.backend = backend or os.environ.get("SPB_GENE_COST", "tensor")
 
     def prepare(self, X: torch.Tensor, metric: str, fixed: bool, centre: Optional[torch.Tensor] = None):
         """Row pre-pass. Returns (operand [n, Gp] fp32 zero-padded to 32 features, rowterm [n] or None).
@@ -212,29 +189,19 @@ class GeneCostBuilder:
         check(self.lib.spb_split_tf32(ptr(op), ptr(hi), ptr(lo), op.numel(), _capi.current_stream_ptr()), "spb_split_tf32")
         return hi, lo
 
-    def cost(self, opA, rtA, opB, rtB, NA, NB, G, metric, prob_type, prob_param, accumulate, GT, ldx, backend=None):
-        backend = backend or self.backend
+    def cost(self, opA, rtA, opB, rtB, NA, NB, G, metric, prob_type, prob_param, accumulate, GT, ldx):
         pp = float(prob_param) if prob_param is not None else 1.0
-        if backend == "tensor":
-            ahi, alo = self._split(opA)
-            bhi, blo = self._split(opB)
-            check(
-                self.lib.spb_gene_cost_tc(
-                    ptr(ahi), ptr(alo), opA.stride(0), ptr(rtA), ptr(bhi), ptr(blo), opB.stride(0), ptr(rtB), NA, NB, G,
-                    _METRIC_CODE[metric], _PROB_CODE[prob_type], pp, 1 if accumulate else 0, ptr(GT), ldx,
-                    _capi.current_stream_ptr(),
-                ),
-                "spb_gene_cost_tc",
-            )
-            self._keep = (ahi, alo, bhi, blo)  # stay alive until the stream has consumed them
-            return
+        ahi, alo = self._split(opA)
+        bhi, blo = self._split(opB)
         check(
-            self.lib.spb_gene_cost(
-                ptr(opA), opA.stride(0), ptr(rtA), ptr(opB), opB.stride(0), ptr(rtB), NA, NB, G, _METRIC_CODE[metric],
-                _PROB_CODE[prob_type], pp, 1 if accumulate else 0, ptr(GT), ldx, _capi.current_stream_ptr(),
+            self.lib.spb_gene_cost_tc(
+                ptr(ahi), ptr(alo), opA.stride(0), ptr(rtA), ptr(bhi), ptr(blo), opB.stride(0), ptr(rtB), NA, NB, G,
+                _METRIC_CODE[metric], _PROB_CODE[prob_type], pp, 1 if accumulate else 0, ptr(GT), ldx,
+                _capi.current_stream_ptr(),
             ),
-            "spb_gene_cost",
+            "spb_gene_cost_tc",
         )
+        self._keep = (ahi, alo, bhi, blo)  # stay alive until the stream has consumed them
 
 
 class Morpho_pairwise:
@@ -348,10 +315,9 @@ class Morpho_pairwise:
         self.materialize_P = materialize_P
         self.compute_mapping = compute_mapping
         self.spatial_sort, self.cull_zero_tiles = spatial_sort, cull_zero_tiles
-        self.use_cuda_graph = os.environ.get("SPB_CUDA_GRAPH", "1") != "0"
         # iterations per captured graph: light iterations (SVI batches, small pairs) are bound by the host's graph launches
         # on a slow host, so several identical iterations ride in one graph; 0 = choose from the pairs per iteration
-        self.graph_unroll = int(os.environ.get("SPB_GRAPH_UNROLL", "0"))
+        self.graph_unroll = 0
         # column-sharded pair: (rank, world, mode) — this process holds the fixed cells [NB * rank / world, NB * (rank + 1) /
         # world) of ONE pair; see alignment/distributed.py:morpho_align_pair_sharded
         self.column_shard = column_shard
@@ -898,16 +864,15 @@ class Morpho_pairwise:
                     cache[key] = t if t.is_pinned() else t.pin_memory()
 
     @staticmethod
-    def _choose_segments(nrb: int, nbb: int, n_sms: int) -> int:
-        """Column segments so that CTAs ~ a multiple of the resident CTA slots (n_sms x 2048 / ROW_TILE) and a segment is at most ``SPB_MAX_COLS_PER_CTA`` columns
+    def _choose_segments(nrb: int, nbb: int, n_sms: int, max_cols: int = 4096) -> int:
+        """Column segments so that CTAs ~ a multiple of the resident CTA slots (n_sms x 2048 / ROW_TILE) and a segment is at most ``max_cols`` columns
         (short CTAs keep the tail of the last wave small once culling has shortened the column lists)."""
-        cap = int(os.environ.get("SPB_MAX_COLS_PER_CTA", "4096"))
         max_seg = max(1, nbb // _capi.COL_STAGE)
         slots = n_sms * (2048 // _capi.ROW_TILE)  # resident CTAs of the sweeps
         seg = 1
         for waves in range(1, 256):
             seg = max(1, min(max_seg, (slots * waves) // max(nrb, 1)))
-            if (nbb + seg - 1) // seg <= cap or seg == max_seg:
+            if (nbb + seg - 1) // seg <= max_cols or seg == max_seg:
                 break
         return seg
 
@@ -1064,8 +1029,7 @@ class Morpho_pairwise:
         p.jacobi_ws = None if s["jacobi_ws"] is None else s["jacobi_ws"].data_ptr()
         p.colmask = s["colmask"].data_ptr() if "colmask" in s else None
         # K^T P K contraction: wgmma (3xTF32) above 32 inducing points, exact fp64 SIMT kernel for small K
-        backend = os.environ.get("SPB_GRAM", "auto")
-        if backend == "tensor" or (backend == "auto" and K > 32):
+        if K > 32:
             if "UT_hi" not in self.__dict__.setdefault("_gram", {}) or self._gram["UT_hi"].shape != self._UT.shape:
                 hi, lo = torch.empty_like(self._UT), torch.empty_like(self._UT)
                 mean = torch.empty((K,), dtype=f32, device=dev)
@@ -1288,8 +1252,7 @@ class Morpho_pairwise:
         with torch.cuda.device(self._dev):
             t0 = _time.perf_counter()
             if self.nn_init:
-                with _nvtx("coarse_rigid_alignment"):
-                    self._coarse_rigid_alignment()
+                self._coarse_rigid_alignment()
             # (stream-level waits: a second pair may be running its EM on another stream of this device)
             torch.cuda.current_stream().synchronize()
             self._timing["coarse_rigid_alignment_s"] = _time.perf_counter() - t0
@@ -1304,8 +1267,7 @@ class Morpho_pairwise:
         if not getattr(self, "_host_ready", False):
             self.prepare_host()
         with torch.cuda.device(self._dev):
-            with _nvtx("expression_cost_matrix"):
-                self._build_gene_cost()
+            self._build_gene_cost()
             self._allocate_state()
             check(self._lib.spb_row_update(C.byref(self._params), _capi.current_stream_ptr()), "spb_row_update")
         self._prepared = True
@@ -1325,8 +1287,8 @@ class Morpho_pairwise:
         """Enqueue EM iterations [start, start + n_iter) on the current stream (no host synchronisation).
 
         Runs of iterations of the same phase (rigid-only up to ``nonrigid_start_iter``, with the non-rigid solve after) are
-        replayed from ONE captured CUDA graph of the iteration's launch sequence (``use_cuda_graph``, default on; the
-        iteration index — SVI batch, step size, trace row — is a device counter). Iterations that need host involvement
+        replayed from ONE captured CUDA graph of the iteration's launch sequence (the iteration index — SVI batch, step
+        size, trace row — is a device counter). Iterations that need host involvement
         (history recording, per-sweep events, the posterior capture of the last iteration, K > SPB_MAX_K_FUSED in the
         non-rigid phase) take the plain path.
 
@@ -1341,8 +1303,8 @@ class Morpho_pairwise:
                 last = it == self.max_iter - 1
                 want_P = (self.materialize_P or self.compute_mapping) and last and not (self.return_mapping and self.SVI_mode)
                 nonrigid = it > self.nonrigid_start_iter
-                plain = (hist is not None or sweep_events is not None or want_P or _nvtx.enabled or self.column_shard is not None
-                         or not getattr(self, "use_cuda_graph", True) or (nonrigid and self.K > _capi.MAX_K_FUSED))
+                plain = (hist is not None or sweep_events is not None or want_P or self.column_shard is not None
+                         or (nonrigid and self.K > _capi.MAX_K_FUSED))
                 if not plain:
                     # iterations [it, stop) share the phase and need nothing from the host
                     stop = min(end, self.nonrigid_start_iter + 1) if not nonrigid else end
@@ -1376,11 +1338,7 @@ class Morpho_pairwise:
                 if hist is not None:
                     hist[it].copy_(self._state["XAHat"])
                     self._state["hist_sigma2"][it].copy_(self._state["sc"][:8].view(torch.float64)[0])
-                if _nvtx.enabled:
-                    torch.cuda.nvtx.range_push(f"em_iteration_{it}")
                 self._iteration(it, st, capture_P=want_P, sweep_events=sweep_events)
-                if _nvtx.enabled:
-                    torch.cuda.nvtx.range_pop()
                 it += 1
 
     def _graph_unroll(self) -> int:

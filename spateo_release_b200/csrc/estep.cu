@@ -23,10 +23,10 @@ constexpr int kConsumers = kRowTile / 4;  // consumer threads, 4 consecutive row
 constexpr int kThreads = kConsumers + 32;
 constexpr int kCtas = 2048 / kRowTile;    // resident CTAs per SM the sweeps are built for (96 registers, ~100 KB of shared memory per 1024 rows)
 constexpr int kColF4 = SPB_COLCONST_FLOATS / 4;  // float4 per column constant record (sweep 1 uses the first two)
+constexpr int kColStage = SPB_COL_STAGE;  // columns per pipeline stage (the host sizes column segments in whole stages)
+constexpr int kStages = 3;                // stages of the shared-memory ring
 
-// Pipeline shape: kColStage columns per stage, kStages stages (compile-time variants, chosen by spb_set_sweep_config).
-template <int kColStage, int kStages>
-struct __align__(16) SmemLayoutT {
+struct __align__(16) SmemLayout {
   float tile[kStages][kColStage][kRowTile];  // kColStage x 4 KB per stage
   float4 cols[kStages][kColStage][kColF4];   // per-column constants, pre-duplicated for packed math (80 B / column)
   float red[2][kConsumers / 32][32];         // sweep-1 cross-warp staging
@@ -47,7 +47,6 @@ __device__ __forceinline__ const int32_t* batch_cols(const int32_t* __restrict__
                                                      int NBb) {
   return batch_base ? batch_base + (int64_t)sc->iter * NBb : nullptr;
 }
-template <int kColStage>
 __device__ __forceinline__ ColRange col_range(const int32_t* __restrict__ colcount, int rb, int seg, int nseg) {
   const int count = colcount[rb];
   int cps = (count + nseg - 1) / nseg;
@@ -61,8 +60,7 @@ __device__ __forceinline__ ColRange col_range(const int32_t* __restrict__ colcou
 // One stage = kColStage GT rows (4 KB each) + the columns' constants. Slots past the end of the slice re-read a valid GT
 // row and take the all-zero constant entry at index NBb (the constant arrays are zero-padded), which keeps the consumer
 // loops branch-free.
-template <int kColStage, int kStages>
-__device__ __forceinline__ void producer_loop(SmemLayoutT<kColStage, kStages>& sm, const float* __restrict__ GT, int64_t ldx,
+__device__ __forceinline__ void producer_loop(SmemLayout& sm, const float* __restrict__ GT, int64_t ldx,
                                               const int32_t* __restrict__ col_index, const int32_t* __restrict__ list,
                                               const float* __restrict__ colsrc, int col_floats, int i0, ColRange cr,
                                               int NBb, int lane) {
@@ -193,8 +191,8 @@ __device__ __forceinline__ RowRegs load_rows(const float* __restrict__ XA, int64
 // sweep 1, one pipeline stage: per column the four partial sums of this thread's 4 rows (index v * kColStage + jj)
 // sweep 1, a stage whose columns are "spatially dead" for this row block (exp2(c_s d) flushes to 0 for every pair: the narrow
 // spatial posterior has no mass here): only the two sums of the sigma2 / full posteriors are formed — half the MUFU work.
-template <int kColStage, int kStages, int kDim = 3>
-__device__ __forceinline__ void sweep1_stage_q(const SmemLayoutT<kColStage, kStages>& sm, int s, int tid, const RowRegs& R,
+template <int kDim = 3>
+__device__ __forceinline__ void sweep1_stage_q(const SmemLayout& sm, int s, int tid, const RowRegs& R,
                                                u64 CQ, float (&acc)[2 * kColStage]) {
 #pragma unroll
   for (int jj = 0; jj < kColStage; ++jj) {
@@ -209,8 +207,8 @@ __device__ __forceinline__ void sweep1_stage_q(const SmemLayoutT<kColStage, kSta
   }
 }
 
-template <int kColStage, int kStages, int kDim = 3>
-__device__ __forceinline__ void sweep1_stage(const SmemLayoutT<kColStage, kStages>& sm, int s, int tid, const RowRegs& R,
+template <int kDim = 3>
+__device__ __forceinline__ void sweep1_stage(const SmemLayout& sm, int s, int tid, const RowRegs& R,
                                              u64 CQ, u64 CS, float (&acc)[4 * kColStage]) {
 #pragma unroll
   for (int jj = 0; jj < kColStage; ++jj) {
@@ -261,8 +259,8 @@ __device__ __forceinline__ u64 keep_ge(u64 w, float tau) {
 }
 
 // kSpatial = false: stage of spatially dead columns (see sweep1_stage_q) — K_NA_spatial receives exact zeros from them
-template <int kColStage, int kStages, bool kSparse, int kDim = 3, bool kSpatial = true>
-__device__ __forceinline__ void sweep2_stage(const SmemLayoutT<kColStage, kStages>& sm, int s, int tid, const RowRegs& R,
+template <bool kSparse, int kDim = 3, bool kSpatial = true>
+__device__ __forceinline__ void sweep2_stage(const SmemLayout& sm, int s, int tid, const RowRegs& R,
                                              u64 CQ, u64 CS, S2Acc& A) {
 #pragma unroll
   for (int jj = 0; jj < kColStage; ++jj) {
@@ -305,18 +303,6 @@ __device__ __forceinline__ void sweep2_stage(const SmemLayoutT<kColStage, kStage
   }
 }
 
-// diagnostic stages (spb_set_sweep_config debug modes): kDbg 1 = stream only (one add per GT value), used to measure the
-// bulk-copy pipeline alone; the full math on a never-refilled ring (kDbg 2) measures the arithmetic alone.
-template <int kColStage, int kStages>
-__device__ __forceinline__ void stream_only_stage(const SmemLayoutT<kColStage, kStages>& sm, int s, int tid, S2Acc& A) {
-#pragma unroll
-  for (int jj = 0; jj < kColStage; ++jj) {
-    const ulonglong2 g = *reinterpret_cast<const ulonglong2*>(&sm.tile[s][jj][tid * 4]);
-    A.ka = add2(A.ka, g.x);
-    A.kb = add2(A.kb, g.y);
-  }
-}
-
 __device__ __forceinline__ float sqdist(float x0, float x1, float x2, const float4& y) {
   const float d0 = x0 - y.x, d1 = x1 - y.y, d2 = x2 - y.z;
   return fmaf(d2, d2, fmaf(d1, d1, d0 * d0));
@@ -325,20 +311,19 @@ __device__ __forceinline__ float sqdist(float x0, float x1, float x2, const floa
 // ---------------------------------------------------------------------------------------------------------------------
 // sweep 1: column sums
 // ---------------------------------------------------------------------------------------------------------------------
-template <int kColStage, int kStages, int kMinBlocks, int kDim = 3>
-__global__ void __launch_bounds__(kThreads, kMinBlocks)
+template <int kDim = 3>
+__global__ void __launch_bounds__(kThreads, kCtas)
 estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __restrict__ batch_base,
                     const float* __restrict__ colgeom, const float* __restrict__ XA, const float* __restrict__ lm,
                     const float* __restrict__ mm, const spb_scalars* __restrict__ sc, float* __restrict__ colpart,
                     int NBb, int nbb_pad, const int32_t* __restrict__ collist, const int32_t* __restrict__ colcount,
                     const int32_t* __restrict__ colsplit) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  using Smem = SmemLayoutT<kColStage, kStages>;
-  Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
+  SmemLayout& sm = *reinterpret_cast<SmemLayout*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int rb = blockIdx.x, seg = blockIdx.y;
   const int i0 = rb * kRowTile;
-  const ColRange cr = col_range<kColStage>(colcount, rb, seg, gridDim.y);
+  const ColRange cr = col_range(colcount, rb, seg, gridDim.y);
   const int32_t* list = collist + (int64_t)rb * nbb_pad;
   const int32_t* col_index = batch_cols(batch_base, sc, NBb);
   const int split = colsplit[rb];  // list positions >= split: spatially dead columns
@@ -353,7 +338,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   __syncthreads();
 
   if (warp == kConsumers / 32) {
-    producer_loop<kColStage, kStages>(sm, GT, ldx, col_index, list, colgeom, 8, i0, cr, NBb, lane);
+    producer_loop(sm, GT, ldx, col_index, list, colgeom, 8, i0, cr, NBb, lane);
     return;
   }
   // ---- consumers: 4 rows per thread = 2 packed row pairs ----
@@ -370,7 +355,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
       // all columns of the stage are spatially dead: sums 0 and 1 are exact zeros, only 2 and 3 are computed and reduced
       constexpr int NQ = 2 * kColStage;
       float acc[NQ];
-      sweep1_stage_q<kColStage, kStages, kDim>(sm, s, tid, R, CQ, acc);
+      sweep1_stage_q<kDim>(sm, s, tid, R, CQ, acc);
       __syncwarp();
       if (lane == 0) mbar_arrive(&sm.empty[s]);
       butterfly_reduce<NQ>(acc, lane);
@@ -392,7 +377,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
       continue;
     }
     float acc[NV];
-    sweep1_stage<kColStage, kStages, kDim>(sm, s, tid, R, CQ, CS, acc);
+    sweep1_stage<kDim>(sm, s, tid, R, CQ, CS, acc);
     __syncwarp();
     if (lane == 0) mbar_arrive(&sm.empty[s]);  // stage buffer is free again
     butterfly_reduce<NV>(acc, lane);
@@ -479,21 +464,20 @@ col_finalize_kernel(const float* __restrict__ colpart, const uint32_t* __restric
 // ---------------------------------------------------------------------------------------------------------------------
 // sweep 2: row statistics
 // ---------------------------------------------------------------------------------------------------------------------
-template <int kColStage, int kStages, int kMinBlocks, bool kSparse, int kDbg = 0, int kDim = 3>
-__global__ void __launch_bounds__(kThreads, kMinBlocks)
+template <bool kSparse, int kDim = 3>
+__global__ void __launch_bounds__(kThreads, kCtas)
 estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __restrict__ batch_base,
                     const float* __restrict__ colconst, const float* __restrict__ XA, const float* __restrict__ lm,
                     const spb_scalars* __restrict__ sc, float* __restrict__ rowpart, int NBb, int nbb_pad,
                     const int32_t* __restrict__ collist, const int32_t* __restrict__ colcount,
                     const int32_t* __restrict__ colsplit) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
-  using Smem = SmemLayoutT<kColStage, kStages>;
-  Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
+  SmemLayout& sm = *reinterpret_cast<SmemLayout*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int rb = blockIdx.x, seg = blockIdx.y;
   const int i0 = rb * kRowTile;
   const int split = colsplit[rb];  // list positions >= split: spatially dead columns (no spatial-posterior work)
-  ColRange cr = col_range<kColStage>(colcount, rb, seg, gridDim.y);
+  const ColRange cr = col_range(colcount, rb, seg, gridDim.y);
   const int32_t* list = collist + (int64_t)rb * nbb_pad;
   const int32_t* col_index = batch_cols(batch_base, sc, NBb);
   const int j_begin = cr.begin, j_end = cr.end;
@@ -507,8 +491,7 @@ estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   __syncthreads();
   const int nst = j_begin < j_end ? (j_end - j_begin + kColStage - 1) / kColStage : 0;
   if (warp == kConsumers / 32) {
-    if constexpr (kDbg == 2) cr.end = min(cr.end, cr.begin + kStages * kColStage);  // fill the ring once, never refill
-    if (j_begin < j_end) producer_loop<kColStage, kStages>(sm, GT, ldx, col_index, list, colconst, SPB_COLCONST_FLOATS, i0, cr, NBb, lane);
+    if (j_begin < j_end) producer_loop(sm, GT, ldx, col_index, list, colconst, SPB_COLCONST_FLOATS, i0, cr, NBb, lane);
     return;
   }
   const u64 CQ = pk(sc->c_q, sc->c_q), CS = pk(sc->c_s, sc->c_s);
@@ -518,14 +501,11 @@ estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   A.clear();
   for (int st = 0; st < nst; ++st) {
     const int s = st % kStages;
-    if (kDbg != 2 || st < kStages) mbar_wait(&sm.full[s], (st / kStages) & 1);
-    if constexpr (kDbg == 1) stream_only_stage<kColStage, kStages>(sm, s, tid, A);
-    else if (j_begin + st * kColStage >= split) sweep2_stage<kColStage, kStages, kSparse, kDim, false>(sm, s, tid, R, CQ, CS, A);
-    else sweep2_stage<kColStage, kStages, kSparse, kDim, true>(sm, s, tid, R, CQ, CS, A);
-    if constexpr (kDbg != 2) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.empty[s]);
-    }
+    mbar_wait(&sm.full[s], (st / kStages) & 1);
+    if (j_begin + st * kColStage >= split) sweep2_stage<kSparse, kDim, false>(sm, s, tid, R, CQ, CS, A);
+    else sweep2_stage<kSparse, kDim, true>(sm, s, tid, R, CQ, CS, A);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&sm.empty[s]);
   }
   A.store(rowpart + ((int64_t)seg * 8) * ldx + r, ldx);
 }
@@ -1170,41 +1150,37 @@ row_argmax_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __re
   if (j0 < j1) atomicMax(rowbest + i, best);
 }
 
-int g_sweep_dbg = 0;  // 0 product, 1 stream-only sweep 2, 2 arithmetic-only sweep 2 (diagnostics, spb_set_sweep_config(16 * mode + cfg))
-
-template <int C, int S, int B, int DIM = 3>
+template <int DIM = 3>
 int launch_sweep1(const spb_em_params* p, const int32_t* bidx, cudaStream_t st) {
-  using Smem = SmemLayoutT<C, S>;
   static bool attr_set[SPB_MAX_DEVICES] = {};  // the opt-in is per device (one process may drive several GPUs)
   const int dev_ = spb_current_device();
   if (!attr_set[dev_]) {
-    cudaError_t e = cudaFuncSetAttribute(estep_sweep1_kernel<C, S, B, DIM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem));
+    cudaError_t e = cudaFuncSetAttribute(estep_sweep1_kernel<DIM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmemLayout));
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(estep_sweep1_kernel<C, S, B, DIM>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    e = cudaFuncSetAttribute(estep_sweep1_kernel<DIM>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return (int)e;
     attr_set[dev_] = true;
   }
   dim3 grid(p->ldx / kRowTile, p->seg1);
-  estep_sweep1_kernel<C, S, B, DIM><<<grid, kThreads, sizeof(Smem), st>>>(p->GT, p->ldx, bidx, p->colgeom, p->XAHat, p->lm, p->mm, p->sc,
-                                                                  p->colpart, p->NBb, p->nbb_pad, p->collist, p->colcount, p->colsplit);
+  estep_sweep1_kernel<DIM><<<grid, kThreads, sizeof(SmemLayout), st>>>(p->GT, p->ldx, bidx, p->colgeom, p->XAHat, p->lm, p->mm, p->sc,
+                                                                      p->colpart, p->NBb, p->nbb_pad, p->collist, p->colcount, p->colsplit);
   return 0;
 }
 
-template <int C, int S, int B, bool SP, int DBG = 0, int DIM = 3>
+template <bool SP, int DIM = 3>
 int launch_sweep2(const spb_em_params* p, const int32_t* bidx, cudaStream_t st) {
-  using Smem = SmemLayoutT<C, S>;
   static bool attr_set[SPB_MAX_DEVICES] = {};  // the opt-in is per device (one process may drive several GPUs)
   const int dev_ = spb_current_device();
   if (!attr_set[dev_]) {
-    cudaError_t e = cudaFuncSetAttribute(estep_sweep2_kernel<C, S, B, SP, DBG, DIM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem));
+    cudaError_t e = cudaFuncSetAttribute(estep_sweep2_kernel<SP, DIM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmemLayout));
     if (e != cudaSuccess) return (int)e;
-    e = cudaFuncSetAttribute(estep_sweep2_kernel<C, S, B, SP, DBG, DIM>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    e = cudaFuncSetAttribute(estep_sweep2_kernel<SP, DIM>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return (int)e;
     attr_set[dev_] = true;
   }
   dim3 grid(p->ldx / kRowTile, p->seg2);
-  estep_sweep2_kernel<C, S, B, SP, DBG, DIM><<<grid, kThreads, sizeof(Smem), st>>>(p->GT, p->ldx, bidx, p->colconst, p->XAHat, p->lm, p->sc,
-                                                                  p->rowpart, p->NBb, p->nbb_pad, p->collist, p->colcount, p->colsplit);
+  estep_sweep2_kernel<SP, DIM><<<grid, kThreads, sizeof(SmemLayout), st>>>(p->GT, p->ldx, bidx, p->colconst, p->XAHat, p->lm, p->sc,
+                                                                          p->rowpart, p->NBb, p->nbb_pad, p->collist, p->colcount, p->colsplit);
   return 0;
 }
 
@@ -1218,13 +1194,6 @@ static inline const int32_t* batch_ptr(const spb_em_params* p, int /*iter*/) {
 extern "C" int spb_gather_cols(const spb_em_params* p, int32_t iter, void* stream) {
   gather_cols_kernel<<<(p->NBb + 255) / 256, 256, 0, (cudaStream_t)stream>>>(p->xb4, batch_ptr(p, iter), p->sc, p->NBb, p->colgeom);
   SPB_CHECK_LAUNCH();
-  return 0;
-}
-
-extern "C" int spb_set_sweep_config(int32_t cfg) {
-  const int shape = cfg & 15, dbg = (cfg >> 4) & 15;
-  if (cfg < 0 || shape != 0 || dbg > 2) return SPB_EINVAL;  // one ring shape is built (8 columns x 3 stages); the others lost
-  g_sweep_dbg = dbg;
   return 0;
 }
 
@@ -1258,8 +1227,8 @@ extern "C" int spb_estep_col_lists(const spb_em_params* p, void* stream) {
 extern "C" int spb_estep_sweep1(const spb_em_params* p, int32_t iter, void* stream) {
   int rc;
   // writes the partial column sums of every (row block, listed column) combination; col_finalize reads exactly those (keepmask)
-  if (p->D == 2) rc = launch_sweep1<8, 3, kCtas, 2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else rc = launch_sweep1<8, 3, kCtas>(p, batch_ptr(p, iter), (cudaStream_t)stream);
+  if (p->D == 2) rc = launch_sweep1<2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
+  else rc = launch_sweep1<>(p, batch_ptr(p, iter), (cudaStream_t)stream);
   if (rc) return rc;
   SPB_CHECK_LAUNCH();
   return 0;
@@ -1274,12 +1243,10 @@ extern "C" int spb_col_finalize(const spb_em_params* p, void* stream) {
 
 extern "C" int spb_estep_sweep2(const spb_em_params* p, int32_t iter, void* stream) {
   int rc;
-  if (p->sparse_k > 0 && p->D == 2) rc = launch_sweep2<8, 3, kCtas, true, 0, 2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else if (p->sparse_k > 0) rc = launch_sweep2<8, 3, kCtas, true>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else if (g_sweep_dbg == 1) rc = launch_sweep2<8, 3, kCtas, false, 1>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else if (g_sweep_dbg == 2) rc = launch_sweep2<8, 3, kCtas, false, 2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else if (p->D == 2) rc = launch_sweep2<8, 3, kCtas, false, 0, 2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else rc = launch_sweep2<8, 3, kCtas, false>(p, batch_ptr(p, iter), (cudaStream_t)stream);
+  if (p->sparse_k > 0 && p->D == 2) rc = launch_sweep2<true, 2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
+  else if (p->sparse_k > 0) rc = launch_sweep2<true>(p, batch_ptr(p, iter), (cudaStream_t)stream);
+  else if (p->D == 2) rc = launch_sweep2<false, 2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
+  else rc = launch_sweep2<false>(p, batch_ptr(p, iter), (cudaStream_t)stream);
   if (rc) return rc;
   SPB_CHECK_LAUNCH();
   return 0;

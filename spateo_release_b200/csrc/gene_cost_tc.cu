@@ -1,6 +1,6 @@
 // Expression cost matrix on the Hopper tensor cores (wgmma + TMA + mbarrier), fp32-accurate through a 3xTF32 split:
 //   x = hi + lo  (hi = tf32(x), lo = x - hi),  A.B ~= Ahi.Bhi + Ahi.Blo + Alo.Bhi  accumulated in fp32 registers.
-// Same contract as gene_cost_kernel (gene_cost.cu): GT[j][i] (op)= prob(metric(A_i, B_j)).
+// GT[j][i] (op)= prob(metric(A_i, B_j)); the operands come from the row pre-passes of gene_cost.cu, split by spb_split_tf32.
 //
 // Per CTA (persistent, one per SM): tile = 128 fixed cells (wgmma M, two warpgroups of 64) x 256 moving cells (wgmma N).
 //   warp 8      TMA producer: 2-stage ring, per k-block (32 features = one 128-byte swizzle row) four 2-D tensor-map loads

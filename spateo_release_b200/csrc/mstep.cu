@@ -80,8 +80,8 @@ __global__ void pxb_term_kernel(spb_em_params p) {
   }
 }
 
-// U^T diag(K_NA) U  and  U^T PXB_term with fp64 products (the reference-accurate path of SparseVFC, and of the alignment when
-// SPB_GRAM=simt): 64 x 64 output tiles of the block upper triangle, 256 threads x (4 x 4) register tiles, operands converted to
+// U^T diag(w) U  and  U^T X3 with fp64 products (spb_weighted_gram: the reference-accurate path of SparseVFC above 32 inducing
+// points): 64 x 64 output tiles of the block upper triangle, 256 threads x (4 x 4) register tiles, operands converted to
 // double ONCE while they are staged through shared memory (32 rows of n per chunk), atomics into the K x K accumulator.
 // grid.x = row chunks, grid.y = (kt, lt) tile pairs with kt <= lt.
 constexpr int kGT = 64;        // tile edge
@@ -817,21 +817,13 @@ extern "C" int spb_nonrigid_accumulate(const spb_em_params* p, void* stream) {
     return spb_gram_tc(p->UT_hi, p->UT_lo, p->GB_hi, p->GB_lo, p->ldx, p->NA, p->K, 3, p->UT_mean, p->gram_sums,
                        p->gram_scratch, p->gram_scratch_floats, p->UtWU, p->UtPXB, stream);
   }
-  if (p->K <= kSmallK) {
-    int rows = (p->NA + 295) / 296;
-    rows = ((rows + 127) / 128) * 128;
-    const int nblk = (p->NA + rows - 1) / rows;
-    if ((int64_t)nblk * p->K * (p->K + 3) > p->red_scratch_doubles) return SPB_EINVAL;
-    gram_small_kernel<<<nblk, 256, 0, ST>>>(p->UT, p->ldx, p->NA, p->K, p->K_NA, p->PXB_term, p->UtWU, p->UtPXB, rows,
-                                            p->red_scratch, p->red_counter + 2);
-    SPB_CHECK_LAUNCH();
-    return 0;
-  }
-  const int ntile = (p->K + kGT - 1) / kGT;
-  const int npairs = ntile * (ntile + 1) / 2;
-  const int rows_per_block = gram_rows_per_block(p->NA, npairs);
-  dim3 grid((p->NA + rows_per_block - 1) / rows_per_block, npairs);
-  weighted_gram_kernel<<<grid, 256, 0, ST>>>(p->UT, p->ldx, p->NA, p->K, p->K_NA, p->PXB_term, p->UtWU, p->UtPXB, rows_per_block, ntile);
+  if (p->K > kSmallK) return SPB_EINVAL;  // above 32 inducing points the caller prepares the tensor-core operands
+  int rows = (p->NA + 295) / 296;
+  rows = ((rows + 127) / 128) * 128;
+  const int nblk = (p->NA + rows - 1) / rows;
+  if ((int64_t)nblk * p->K * (p->K + 3) > p->red_scratch_doubles) return SPB_EINVAL;
+  gram_small_kernel<<<nblk, 256, 0, ST>>>(p->UT, p->ldx, p->NA, p->K, p->K_NA, p->PXB_term, p->UtWU, p->UtPXB, rows,
+                                          p->red_scratch, p->red_counter + 2);
   SPB_CHECK_LAUNCH();
   return 0;
 }

@@ -159,13 +159,12 @@ def test_argmax_key_decoding_and_transpose():
     assert t.shape == (2, 3) and np.array_equal(t.row_arg, pi.col_arg) and np.array_equal(t.col_val, pi.row_val)
 
 
-def test_segment_choice_respects_the_column_cap(monkeypatch):
+def test_segment_choice_respects_the_column_cap():
     from spateo_release_b200.alignment.morpho_class import Morpho_pairwise
 
     seg = Morpho_pairwise._choose_segments(98, 100000, 132)  # H100 SXM
     assert (100000 + seg - 1) // seg <= 4096 and seg * 98 >= 296
-    monkeypatch.setenv("SPB_MAX_COLS_PER_CTA", "1024")
-    seg2 = Morpho_pairwise._choose_segments(98, 100000, 132)
+    seg2 = Morpho_pairwise._choose_segments(98, 100000, 132, max_cols=1024)
     assert seg2 > seg and (100000 + seg2 - 1) // seg2 <= 1024
     assert Morpho_pairwise._choose_segments(1, 240, 132) >= 1
 
@@ -231,7 +230,7 @@ def test_solve_RT_by_correspondence_reproduces_reference_links(golden):
 
 def test_graph_unroll_choice():
     """Iterations per captured CUDA graph: 8 for light iterations (default SVI batch of the 100k pair, small pairs), 1 for
-    the heavy full-EM iterations; an explicit value (SPB_GRAPH_UNROLL / attribute) wins."""
+    the heavy full-EM iterations; an explicit ``graph_unroll`` attribute wins."""
     from types import SimpleNamespace
 
     from spateo_release_b200.alignment.morpho_class import Morpho_pairwise
