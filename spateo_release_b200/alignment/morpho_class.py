@@ -90,19 +90,32 @@ def _round_up(x: int, m: int) -> int:
     return ((x + m - 1) // m) * m
 
 
-def morton_order(coords: np.ndarray) -> np.ndarray:
-    """Row permutation that sorts points along a Z-order curve (isotropic quantisation: 16 bits/axis in 2-D, 10 in 3-D)."""
-    c = np.asarray(coords, dtype=np.float64)
-    n, D = c.shape
-    bits = 16 if D == 2 else 10
-    lo = c.min(axis=0)
-    ext = max(float((c.max(axis=0) - lo).max()), 1e-30)
-    q = np.minimum(((c - lo) / ext * (2**bits - 1)).astype(np.uint64), np.uint64(2**bits - 1))
-    code = np.zeros(n, dtype=np.uint64)
-    for b in range(bits):
-        for d in range(D):
-            code |= ((q[:, d] >> np.uint64(b)) & np.uint64(1)) << np.uint64(b * D + d)
-    return np.argsort(code, kind="stable")
+def _kd_groups(c: np.ndarray, idx: np.ndarray, unit: int) -> list:
+    """Split the points ``idx`` (columns of the [D][n] coordinates ``c``) into consecutive groups of ``unit`` rows (the last one may be shorter): each cut goes across the
+    longest extent of the points it splits, after floor(groups / 2) whole groups (a stable sort makes it deterministic)."""
+    out, stack = [], [idx]
+    while stack:  # depth first, left part before right part
+        ix = stack.pop()
+        groups = -(-ix.shape[0] // unit)
+        if groups <= 1:
+            out.append(ix)
+            continue
+        p = c[:, ix]
+        axis = int(np.argmax(p.max(axis=1) - p.min(axis=1)))
+        ix = ix[np.argsort(p[axis], kind="stable")]
+        cut = (groups // 2) * unit
+        stack.append(ix[cut:])
+        stack.append(ix[:cut])
+    return out
+
+
+def kd_order(coords: np.ndarray, tile: int = 512, quarter: int = 128) -> np.ndarray:
+    """Row permutation into compact row blocks: a balanced k-d split of the points into blocks of ``tile`` rows, then of every
+    block into ``quarter``-row parts the same way. Row block k is rows [k tile, (k + 1) tile) of the permuted order; only the
+    last block can be short."""
+    c = np.ascontiguousarray(np.asarray(coords, dtype=np.float64).T)
+    blocks = _kd_groups(c, np.arange(c.shape[1], dtype=np.int64), tile)
+    return np.concatenate([q for b in blocks for q in _kd_groups(c, b, quarter)])
 
 
 def resolve_device(device) -> torch.device:
@@ -211,9 +224,10 @@ class Morpho_pairwise:
     N_A x N_B posterior (40 GB at 100k x 100k) and returns None; every other output is unaffected.
     ``compute_mapping`` — ``self.mapping`` (an ``ArgmaxPi``) receives the row / column maxima of the final posterior from a
     fused kernel, for ``get_optimal_mapping_relationship`` / ``mapping_aligned_coords`` without a dense P.
-    ``spatial_sort`` / ``cull_zero_tiles`` — the moving cells are processed in Morton order so that each row block (SPB_ROW_TILE = 512 cells) is
-    spatially compact, and (row block, fixed cell) tiles whose every pair underflows to exactly 0 in fp32 are skipped;
-    results are bit-identical to the dense sweep (all outputs are returned in the caller's row order).
+    ``spatial_sort`` / ``cull_zero_tiles`` — the moving cells are processed in k-d order (``kd_order``) so that each row block
+    (SPB_ROW_TILE = 512 cells) and each of its four 128-cell quarters is spatially compact, and the (quarter, fixed cell) pairs
+    of rows whose every pair underflows to exactly 0 in fp32 are neither read nor computed; results are bit-identical to the
+    dense sweep in the same row order (all outputs are returned in the caller's row order).
     ``column_shard`` — set by ``morpho_align_pair_sharded``: one pair's fixed cells split over several GPUs.
     Accepted but without effect (memory work-arounds whose results are identical): ``use_chunk``, ``chunk_capacity``,
     ``pre_compute_dist``. ``sparse_calculation_mode`` keeps the top ``sparse_top_k`` posterior entries of every column by an
@@ -770,7 +784,7 @@ class Morpho_pairwise:
     def _set_row_order(self):
         """Processing order of the moving cells (after the coarse initialisation moved them)."""
         if self.spatial_sort and self.NA > _capi.ROW_TILE:
-            self._perm = morton_order(self.coordsA)
+            self._perm = kd_order(self.coordsA, _capi.ROW_TILE, _capi.ROW_TILE // 4)
             self._perm_dev = torch.from_numpy(self._perm).to(self._dev)
         else:
             self._perm, self._perm_dev = None, None
@@ -924,8 +938,9 @@ class Morpho_pairwise:
         seg2 = self._choose_segments(nrb, nbb, n_sms)
         seg_alloc = max(seg2, self._choose_segments(nrb, nbb_alloc, n_sms))
         s["rowpart"] = torch.zeros((seg_alloc, 8, ldx), dtype=f32, device=dev)
-        s["bbox"] = torch.zeros((nrb, 8), dtype=f32, device=dev)
+        s["bbox"] = torch.zeros((nrb, 4, 8), dtype=f32, device=dev)
         s["collist"] = torch.zeros((nrb, self._nbb_pad), dtype=torch.int32, device=dev)
+        s["colquarters"] = torch.zeros((nrb, self._nbb_pad), dtype=torch.uint8, device=dev)
         s["colcount"] = torch.zeros((nrb,), dtype=torch.int32, device=dev)
         s["colsplit"] = torch.zeros((nrb,), dtype=torch.int32, device=dev)
         if self.sparse_calculation_mode:
@@ -1020,7 +1035,7 @@ class Morpho_pairwise:
         p.GT, p.UT = ptr(self._GT).value, ptr(self._UT).value
         for name in ("xa", "xb4", "Gamma", "kappa", "batch_idx", "alpha", "SigmaDiag", "lm", "mm", "VnA", "RnA", "XAHat",
                      "K_NA", "K_NA_spatial", "K_NA_sigma2", "PXB", "PXB_term", "K_NB", "colgeom", "colconst", "colpart", "keepmask",
-                     "rowpart", "bbox", "collist", "colcount", "colsplit", "UtWU", "UtPXB", "SigmaInv", "Sigma", "Coff", "moments", "sc",
+                     "rowpart", "bbox", "collist", "colquarters", "colcount", "colsplit", "UtWU", "UtPXB", "SigmaInv", "Sigma", "Coff", "moments", "sc",
                      "trace_buf"):
             t = s[name]
             setattr(p, name, None if t is None else t.data_ptr())

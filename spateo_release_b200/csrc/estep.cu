@@ -25,11 +25,14 @@ constexpr int kCtas = 2048 / kRowTile;    // resident CTAs per SM the sweeps are
 constexpr int kColF4 = SPB_COLCONST_FLOATS / 4;  // float4 per column constant record (sweep 1 uses the first two)
 constexpr int kColStage = SPB_COL_STAGE;  // columns per pipeline stage (the host sizes column segments in whole stages)
 constexpr int kStages = 3;                // stages of the shared-memory ring
+constexpr int kQuarter = 32 * 4;          // rows of one consumer warp: the granularity of the culling within a row block
+static_assert(kColStage == 8, "one 64-bit word holds the quarter masks of a stage");
 
 struct __align__(16) SmemLayout {
   float tile[kStages][kColStage][kRowTile];  // kColStage x 4 KB per stage
   float4 cols[kStages][kColStage][kColF4];   // per-column constants, pre-duplicated for packed math (80 B / column)
   float red[2][kConsumers / 32][32];         // sweep-1 cross-warp staging
+  uint64_t quarters[kStages];                // byte jj: live quarters of the stage's column jj (colquarters)
   uint64_t full[kStages];
   uint64_t empty[kStages];
 };
@@ -57,30 +60,53 @@ __device__ __forceinline__ ColRange col_range(const int32_t* __restrict__ colcou
   return r;
 }
 
-// One stage = kColStage GT rows (4 KB each) + the columns' constants. Slots past the end of the slice re-read a valid GT
-// row and take the all-zero constant entry at index NBb (the constant arrays are zero-padded), which keeps the consumer
-// loops branch-free.
+// One stage = the live quarters (512 B each) of kColStage GT rows + the columns' constants. A column's live quarters
+// (colquarters) are copied as one bulk copy per run of adjacent quarters (a 4-bit mask has at most two runs); the other
+// quarters of the slot keep stale data that the owning consumer warp never reads. Slots past the end of the slice have
+// no live quarter and take the all-zero constant entry at index NBb (the constant arrays are zero-padded). The stage's
+// masks go to sm.quarters before the arrive on the full barrier, which publishes them with the copies.
 __device__ __forceinline__ void producer_loop(SmemLayout& sm, const float* __restrict__ GT, int64_t ldx,
                                               const int32_t* __restrict__ col_index, const int32_t* __restrict__ list,
-                                              const float* __restrict__ colsrc, int col_floats, int i0, ColRange cr,
-                                              int NBb, int lane) {
+                                              const uint8_t* __restrict__ quarters, const float* __restrict__ colsrc,
+                                              int col_floats, int i0, ColRange cr, int NBb, int lane) {
   const int nst = (cr.end - cr.begin + kColStage - 1) / kColStage;
   for (int st = 0; st < nst; ++st) {
     const int s = st % kStages;
     if (st >= kStages) mbar_wait(&sm.empty[s], ((st / kStages) - 1) & 1);
     const int pb = cr.begin + st * kColStage;
-    if (lane == 0) mbar_expect_tx(&sm.full[s], (uint32_t)(kColStage * kRowTile * 4 + kColStage * col_floats * 4));
+    const bool slot = lane < kColStage, live = slot && pb + lane < cr.end;
+    const uint32_t qm = live ? quarters[pb + lane] : 0u;
+    const uint32_t bytes = slot ? __popc(qm) * kQuarter * 4 + col_floats * 4 : 0u;
+    const uint32_t total = __reduce_add_sync(0xffffffffu, bytes);
+    const uint32_t lo = __reduce_or_sync(0xffffffffu, lane < 4 ? qm << (8 * lane) : 0u);
+    const uint32_t hi = __reduce_or_sync(0xffffffffu, (lane >= 4 && slot) ? qm << (8 * (lane - 4)) : 0u);
+    if (lane == 0) {
+      sm.quarters[s] = ((uint64_t)hi << 32) | lo;
+      mbar_expect_tx(&sm.full[s], total);
+    }
     __syncwarp();
-    if (lane < kColStage) {
-      const bool live = pb + lane < cr.end;
-      const int j = live ? list[pb + lane] : NBb;          // NBb = zero-constant pad entry
-      const int jr = live ? j : list[cr.end - 1];          // any valid GT row for pad slots
-      const int64_t row = col_index ? (int64_t)col_index[jr] : (int64_t)jr;
-      bulk_g2s(&sm.tile[s][lane][0], GT + row * ldx + i0, kRowTile * 4, &sm.full[s]);
+    if (slot) {
+      const int j = live ? list[pb + lane] : NBb;  // NBb = zero-constant pad entry
+      if (qm != 0u) {
+        const int64_t row = col_index ? (int64_t)col_index[j] : (int64_t)j;
+        const float* src = GT + row * ldx + i0;
+        for (uint32_t m = qm; m != 0u;) {
+          const int q0 = __ffs(m) - 1;
+          const int len = __ffs(~(m >> q0)) - 1;  // length of the run of set bits starting at q0
+          bulk_g2s(&sm.tile[s][lane][q0 * kQuarter], src + q0 * kQuarter, len * kQuarter * 4, &sm.full[s]);
+          m &= ~(((1u << len) - 1u) << q0);
+        }
+      }
       bulk_g2s(&sm.cols[s][lane][0], colsrc + (int64_t)j * col_floats, col_floats * 4, &sm.full[s]);
     }
   }
 }
+
+// A consumer warp skips a column whose quarter bit is clear (colquarters): every pair of its 128 rows with that column has
+// ex2(c_q d + lm) = +0 and ex2(c_s d) = +0 in fp32 (c_q dmin^2 < -127 for the quarter's box, lm <= 0 because alpha < 1 and
+// SigmaDiag >= 0, c_s <= c_q < 0), so sweep 1 would have reduced exact zeros and sweep 2 would have added exact zeros (an
+// accumulator that starts at +0 is never -0, so x + 0 = x). Skipping is therefore bit-identical.
+__device__ __forceinline__ bool quarter_live(uint64_t wq, int jj) { return (wq >> (8 * jj)) & 1u; }
 
 // ---- fp32 pairs: two moving cells per value. Hopper has no packed fp32x2 instructions, so every pair operation is two
 // scalar operations with explicit round-to-nearest (no contraction: the same bits as a packed add / mul / fma) ----------
@@ -193,9 +219,13 @@ __device__ __forceinline__ RowRegs load_rows(const float* __restrict__ XA, int64
 // spatial posterior has no mass here): only the two sums of the sigma2 / full posteriors are formed — half the MUFU work.
 template <int kDim = 3>
 __device__ __forceinline__ void sweep1_stage_q(const SmemLayout& sm, int s, int tid, const RowRegs& R,
-                                               u64 CQ, float (&acc)[2 * kColStage]) {
+                                               u64 CQ, uint64_t wq, float (&acc)[2 * kColStage]) {
 #pragma unroll
   for (int jj = 0; jj < kColStage; ++jj) {
+    if (!quarter_live(wq, jj)) {
+      acc[0 * kColStage + jj] = acc[1 * kColStage + jj] = 0.f;
+      continue;
+    }
     const ulonglong2 ya = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][0]);
     const ulonglong2 yb = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][1]);
     const ulonglong2 g = *reinterpret_cast<const ulonglong2*>(&sm.tile[s][jj][tid * 4]);
@@ -209,9 +239,13 @@ __device__ __forceinline__ void sweep1_stage_q(const SmemLayout& sm, int s, int 
 
 template <int kDim = 3>
 __device__ __forceinline__ void sweep1_stage(const SmemLayout& sm, int s, int tid, const RowRegs& R,
-                                             u64 CQ, u64 CS, float (&acc)[4 * kColStage]) {
+                                             u64 CQ, u64 CS, uint64_t wq, float (&acc)[4 * kColStage]) {
 #pragma unroll
   for (int jj = 0; jj < kColStage; ++jj) {
+    if (!quarter_live(wq, jj)) {
+      acc[0 * kColStage + jj] = acc[1 * kColStage + jj] = acc[2 * kColStage + jj] = acc[3 * kColStage + jj] = 0.f;
+      continue;
+    }
     const ulonglong2 ya = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][0]);  // (y0,y0) (y1,y1)
     const ulonglong2 yb = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][1]);  // (y2,y2) (0,0)
     const ulonglong2 g = *reinterpret_cast<const ulonglong2*>(&sm.tile[s][jj][tid * 4]);
@@ -261,9 +295,10 @@ __device__ __forceinline__ u64 keep_ge(u64 w, float tau) {
 // kSpatial = false: stage of spatially dead columns (see sweep1_stage_q) — K_NA_spatial receives exact zeros from them
 template <bool kSparse, int kDim = 3, bool kSpatial = true>
 __device__ __forceinline__ void sweep2_stage(const SmemLayout& sm, int s, int tid, const RowRegs& R,
-                                             u64 CQ, u64 CS, S2Acc& A) {
+                                             u64 CQ, u64 CS, uint64_t wq, S2Acc& A) {
 #pragma unroll
   for (int jj = 0; jj < kColStage; ++jj) {
+    if (!quarter_live(wq, jj)) continue;
     const ulonglong2 c0 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][0]);  // (y0,y0) (y1,y1)
     const ulonglong2 c1 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][1]);  // (y2,y2) (a,a)
     const ulonglong2 c2 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][2]);  // (b,b)  (c,c)
@@ -316,8 +351,8 @@ __global__ void __launch_bounds__(kThreads, kCtas)
 estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __restrict__ batch_base,
                     const float* __restrict__ colgeom, const float* __restrict__ XA, const float* __restrict__ lm,
                     const float* __restrict__ mm, const spb_scalars* __restrict__ sc, float* __restrict__ colpart,
-                    int NBb, int nbb_pad, const int32_t* __restrict__ collist, const int32_t* __restrict__ colcount,
-                    const int32_t* __restrict__ colsplit) {
+                    int NBb, int nbb_pad, const int32_t* __restrict__ collist, const uint8_t* __restrict__ colquarters,
+                    const int32_t* __restrict__ colcount, const int32_t* __restrict__ colsplit) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   SmemLayout& sm = *reinterpret_cast<SmemLayout*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -325,6 +360,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   const int i0 = rb * kRowTile;
   const ColRange cr = col_range(colcount, rb, seg, gridDim.y);
   const int32_t* list = collist + (int64_t)rb * nbb_pad;
+  const uint8_t* quarters = colquarters + (int64_t)rb * nbb_pad;
   const int32_t* col_index = batch_cols(batch_base, sc, NBb);
   const int split = colsplit[rb];  // list positions >= split: spatially dead columns
   if (cr.begin >= cr.end) return;
@@ -338,7 +374,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   __syncthreads();
 
   if (warp == kConsumers / 32) {
-    producer_loop(sm, GT, ldx, col_index, list, colgeom, 8, i0, cr, NBb, lane);
+    producer_loop(sm, GT, ldx, col_index, list, quarters, colgeom, 8, i0, cr, NBb, lane);
     return;
   }
   // ---- consumers: 4 rows per thread = 2 packed row pairs ----
@@ -351,11 +387,12 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
     const int pb = cr.begin + st * kColStage;
     constexpr int NV = 4 * kColStage;  // partial sums per thread per stage, index v * kColStage + jj
     const int buf = st & 1;
+    const uint64_t wq = sm.quarters[s] >> warp;  // bit 8 jj: this warp's quarter of column jj is live
     if (pb >= split) {
       // all columns of the stage are spatially dead: sums 0 and 1 are exact zeros, only 2 and 3 are computed and reduced
       constexpr int NQ = 2 * kColStage;
       float acc[NQ];
-      sweep1_stage_q<kDim>(sm, s, tid, R, CQ, acc);
+      sweep1_stage_q<kDim>(sm, s, tid, R, CQ, wq, acc);
       __syncwarp();
       if (lane == 0) mbar_arrive(&sm.empty[s]);
       butterfly_reduce<NQ>(acc, lane);
@@ -377,7 +414,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
       continue;
     }
     float acc[NV];
-    sweep1_stage<kDim>(sm, s, tid, R, CQ, CS, acc);
+    sweep1_stage<kDim>(sm, s, tid, R, CQ, CS, wq, acc);
     __syncwarp();
     if (lane == 0) mbar_arrive(&sm.empty[s]);  // stage buffer is free again
     butterfly_reduce<NV>(acc, lane);
@@ -469,8 +506,8 @@ __global__ void __launch_bounds__(kThreads, kCtas)
 estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __restrict__ batch_base,
                     const float* __restrict__ colconst, const float* __restrict__ XA, const float* __restrict__ lm,
                     const spb_scalars* __restrict__ sc, float* __restrict__ rowpart, int NBb, int nbb_pad,
-                    const int32_t* __restrict__ collist, const int32_t* __restrict__ colcount,
-                    const int32_t* __restrict__ colsplit) {
+                    const int32_t* __restrict__ collist, const uint8_t* __restrict__ colquarters,
+                    const int32_t* __restrict__ colcount, const int32_t* __restrict__ colsplit) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   SmemLayout& sm = *reinterpret_cast<SmemLayout*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -479,6 +516,7 @@ estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   const int split = colsplit[rb];  // list positions >= split: spatially dead columns (no spatial-posterior work)
   const ColRange cr = col_range(colcount, rb, seg, gridDim.y);
   const int32_t* list = collist + (int64_t)rb * nbb_pad;
+  const uint8_t* quarters = colquarters + (int64_t)rb * nbb_pad;
   const int32_t* col_index = batch_cols(batch_base, sc, NBb);
   const int j_begin = cr.begin, j_end = cr.end;
   if (tid == 0) {
@@ -491,7 +529,7 @@ estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   __syncthreads();
   const int nst = j_begin < j_end ? (j_end - j_begin + kColStage - 1) / kColStage : 0;
   if (warp == kConsumers / 32) {
-    if (j_begin < j_end) producer_loop(sm, GT, ldx, col_index, list, colconst, SPB_COLCONST_FLOATS, i0, cr, NBb, lane);
+    if (j_begin < j_end) producer_loop(sm, GT, ldx, col_index, list, quarters, colconst, SPB_COLCONST_FLOATS, i0, cr, NBb, lane);
     return;
   }
   const u64 CQ = pk(sc->c_q, sc->c_q), CS = pk(sc->c_s, sc->c_s);
@@ -502,8 +540,9 @@ estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   for (int st = 0; st < nst; ++st) {
     const int s = st % kStages;
     mbar_wait(&sm.full[s], (st / kStages) & 1);
-    if (j_begin + st * kColStage >= split) sweep2_stage<kSparse, kDim, false>(sm, s, tid, R, CQ, CS, A);
-    else sweep2_stage<kSparse, kDim, true>(sm, s, tid, R, CQ, CS, A);
+    const uint64_t wq = sm.quarters[s] >> warp;
+    if (j_begin + st * kColStage >= split) sweep2_stage<kSparse, kDim, false>(sm, s, tid, R, CQ, CS, wq, A);
+    else sweep2_stage<kSparse, kDim, true>(sm, s, tid, R, CQ, CS, wq, A);
     __syncwarp();
     if (lane == 0) mbar_arrive(&sm.empty[s]);
   }
@@ -612,10 +651,10 @@ row_stats_p2p_kernel(const uint64_t* __restrict__ peer_stat, int parity, int ran
   grid_reduce_ordered<4>(v, red_scratch, red_counter, sc->sums, false);
 }
 
-// bounding box of the current positions of each row block (valid rows only)
+// bounding box of the current positions of each 128-row quarter of each row block (valid rows only): warp w reduces the
+// rows of consumer warp w of the sweeps
 __global__ void __launch_bounds__(kConsumers) block_bounds_kernel(const float* __restrict__ XA, int ldx, int NA,
                                                                   float* __restrict__ bbox) {
-  __shared__ float red[6][kConsumers / 32];
   const int rb = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f};
   for (int q = 0; q < 4; ++q) {
@@ -637,47 +676,74 @@ __global__ void __launch_bounds__(kConsumers) block_bounds_kernel(const float* _
       hi[d] = fmaxf(hi[d], __shfl_xor_sync(0xffffffffu, hi[d], o));
     }
     if (lane == 0) {
-      red[d][warp] = lo[d];
-      red[3 + d][warp] = hi[d];
+      bbox[(rb * 4 + warp) * 8 + d] = lo[d];
+      bbox[(rb * 4 + warp) * 8 + 3 + d] = hi[d];
     }
   }
-  __syncthreads();
-  if (threadIdx.x < 6) {
-    float v = red[threadIdx.x][0];
-    for (int w = 1; w < kConsumers / 32; ++w) v = threadIdx.x < 3 ? fminf(v, red[threadIdx.x][w]) : fmaxf(v, red[threadIdx.x][w]);
-    bbox[rb * 8 + threadIdx.x] = v;
+}
+
+__device__ __forceinline__ float box_dist2(const float (&lo)[3], const float (&hi)[3], const float (&y)[3]) {
+  float d2 = 0.f;
+#pragma unroll
+  for (int d = 0; d < 3; ++d) {
+    const float g = fmaxf(fmaxf(lo[d] - y[d], y[d] - hi[d]), 0.f);
+    d2 = fmaf(g, g, d2);
   }
+  return d2;
 }
 
 // Per row block: order-preserving compaction of the columns that are not provably zero for every row of the block.
 // A column j is dropped when c_q * dmin^2 < -127 (log2 domain, with a 1e-5 relative safety margin), dmin = distance from
 // y_j to the block's bounding box: then ex2(c_q d + lm) and ex2(c_s d) flush to +0 for every pair of the block (lm <= 0,
-// c_s <= c_q < 0), so the dropped pairs would have added exact zeros.
-// One CTA per row block, 32 warps, each warp owns a contiguous range of columns: pass 1 evaluates the test once (the keep
-// bits go to shared memory), one block barrier turns the per-warp counts into offsets, pass 2 scatters. The keep bits are also
-// published (keepmask): col_finalize folds only the partial column sums that sweep 1 wrote, so the dropped (row block, column)
-// combinations are neither zeroed (a 157-313 MB write per iteration) nor read.
+// c_s <= c_q < 0), so the dropped pairs would have added exact zeros. The same test against the box of each 128-row quarter
+// gives the listed column's quarter mask (colquarters): the sweeps read and compute only the live quarters of a column.
+// The list itself is built from the block's box, so the list, its live / dead split and the column segments of the sweeps
+// do not depend on the quarter masks, and neither does the order in which any sum is formed.
+// One CTA per row block, 32 warps, each warp owns a contiguous range of columns: pass 1 evaluates the block test once (the
+// keep bits go to shared memory), one block barrier turns the per-warp counts into offsets, pass 2 scatters the listed
+// columns with their quarter masks. The keep bits are also published (keepmask): col_finalize folds only the partial column
+// sums that sweep 1 wrote, so the dropped (row block, column) combinations are neither zeroed (a 157-313 MB write per
+// iteration) nor read.
 constexpr int kListThreads = 1024;
 // geom: one record per column, `gstride` floats apart, coordinate d at float offset d * gstep (the 16-byte xb4 records when the
 // columns are all fixed cells: half the L2 traffic of the duplicated colgeom layout, which every row block re-reads in full)
+__device__ __forceinline__ void load_col(const float* __restrict__ geom, int gstride, int gstep, int j, bool in, int cull,
+                                         float (&y)[3]) {
+  const float* p = geom + (int64_t)(in ? j : 0) * gstride;
+  if (gstride == 4) {  // one 16-byte load per column
+    const float4 v = cull ? *reinterpret_cast<const float4*>(p) : make_float4(0.f, 0.f, 0.f, 0.f);
+    y[0] = v.x, y[1] = v.y, y[2] = v.z;
+  } else {
+#pragma unroll
+    for (int d = 0; d < 3; ++d) y[d] = cull ? p[d * gstep] : 0.f;
+  }
+}
+
 __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const float* __restrict__ bbox, const float* __restrict__ geom,
                                                                        int gstride, int gstep,
                                                                        int NBb, spb_scalars* __restrict__ sc, int cull,
-                                                                       int32_t* __restrict__ collist, int32_t* __restrict__ colcount,
-                                                                       int32_t* __restrict__ colsplit, int nbb_pad,
-                                                                       uint32_t* __restrict__ colmask, uint32_t* __restrict__ keepmask,
-                                                                       int kstride) {
+                                                                       int32_t* __restrict__ collist, uint8_t* __restrict__ colquarters,
+                                                                       int32_t* __restrict__ colcount, int32_t* __restrict__ colsplit,
+                                                                       int nbb_pad, uint32_t* __restrict__ colmask,
+                                                                       uint32_t* __restrict__ keepmask, int kstride) {
   extern __shared__ uint32_t keep_bits[];  // [2][nwords]: one word per 32 columns — kept at all | spatially live
   __shared__ int warp_cnt[2][32];
+  __shared__ int live_quarters;
   const int rb = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const float cq = sc->c_q * (1.0f - 1e-5f);
   const float cs = sc->c_s * (1.0f - 1e-5f);  // c_s = c_q * sigma2_variance <= c_q: the spatial weight dies first
-  float lo[3], hi[3];
+  float qlo[4][3], qhi[4][3], lo[3], hi[3];   // quarter boxes and the block's box (their union)
 #pragma unroll
-  for (int d = 0; d < 3; ++d) {
-    lo[d] = bbox[rb * 8 + d];
-    hi[d] = bbox[rb * 8 + 3 + d];
+  for (int q = 0; q < 4; ++q) {
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+      qlo[q][d] = bbox[(rb * 4 + q) * 8 + d];
+      qhi[q][d] = bbox[(rb * 4 + q) * 8 + 3 + d];
+      lo[d] = q ? fminf(lo[d], qlo[q][d]) : qlo[q][d];
+      hi[d] = q ? fmaxf(hi[d], qhi[q][d]) : qhi[q][d];
+    }
   }
+  if (threadIdx.x == 0) live_quarters = 0;
   const int nwords = (NBb + 31) / 32;
   uint32_t* live_bits = keep_bits + nwords;
   const int wpw = (nwords + 31) / 32;  // words per warp
@@ -689,15 +755,7 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
 #pragma unroll
     for (int u = 0; u < kU; ++u) {
       const int j = (wb + u) * 32 + lane;
-      const bool in = (wb + u < w1) && j < NBb;
-      const float* y = geom + (int64_t)(in ? j : 0) * gstride;
-      if (gstride == 4) {  // one 16-byte load per column
-        const float4 v = cull ? *reinterpret_cast<const float4*>(y) : make_float4(0.f, 0.f, 0.f, 0.f);
-        yy[u][0] = v.x, yy[u][1] = v.y, yy[u][2] = v.z;
-      } else {
-#pragma unroll
-        for (int d = 0; d < 3; ++d) yy[u][d] = cull ? y[d * gstep] : 0.f;
-      }
+      load_col(geom, gstride, gstep, j, (wb + u < w1) && j < NBb, cull, yy[u]);
     }
 #pragma unroll
     for (int u = 0; u < kU; ++u) {
@@ -708,12 +766,7 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
       if (j < NBb) {
         keep = live = true;
         if (cull) {
-          float d2 = 0.f;
-#pragma unroll
-          for (int d = 0; d < 3; ++d) {
-            const float g = fmaxf(fmaxf(lo[d] - yy[u][d], yy[u][d] - hi[d]), 0.f);
-            d2 = fmaf(g, g, d2);
-          }
+          const float d2 = box_dist2(lo, hi, yy[u]);
           keep = cq * d2 >= -127.0f;
           live = cs * d2 >= -127.0f;  // implies keep
         }
@@ -749,22 +802,43 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
   }
   off_dead += total_live;  // the spatially dead columns follow the live ones in the list
   int32_t* list = collist + (int64_t)rb * nbb_pad;
+  uint8_t* qlist = colquarters + (int64_t)rb * nbb_pad;
+  int nq = 0;  // live quarters of this lane's listed columns
+  float ynext[3];
+  if (w0 < w1) load_col(geom, gstride, gstep, w0 * 32 + lane, w0 * 32 + lane < NBb, cull, ynext);
   for (int wd = w0; wd < w1; ++wd) {
     const uint32_t bits = keep_bits[wd], lbits = live_bits[wd], dbits = bits & ~lbits;
     const int j = wd * 32 + lane;
+    const float y[3] = {ynext[0], ynext[1], ynext[2]};
+    if (wd + 1 < w1) load_col(geom, gstride, gstep, j + 32, j + 32 < NBb, cull, ynext);  // next word's column, in flight
     const uint32_t below = (1u << lane) - 1u;
-    if ((lbits >> lane) & 1u) list[off_live + __popc(lbits & below)] = j;
-    else if ((dbits >> lane) & 1u) list[off_dead + __popc(dbits & below)] = j;
+    int pos = -1;
+    if ((lbits >> lane) & 1u) pos = off_live + __popc(lbits & below);
+    else if ((dbits >> lane) & 1u) pos = off_dead + __popc(dbits & below);
+    if (pos >= 0) {
+      uint32_t qm = 0xFu;  // without culling every quarter of every column is read
+      if (cull) {
+        qm = 0u;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) qm |= (cq * box_dist2(qlo[q], qhi[q], y) >= -127.0f) ? 1u << q : 0u;
+      }
+      list[pos] = j;
+      qlist[pos] = (uint8_t)qm;
+      nq += __popc(qm);
+    }
     if (lane == 0) keepmask[(int64_t)rb * kstride + wd] = bits;  // col_finalize folds only the listed (row block, column) partials
     if (((bits >> lane) & 1u) && colmask != nullptr && rb < 32 * SPB_COLMASK_WORDS)
       atomicOr(colmask + (int64_t)j * SPB_COLMASK_WORDS + (rb >> 5), 1u << (rb & 31));
     off_live += __popc(lbits);
     off_dead += __popc(dbits);
   }
+  nq = __reduce_add_sync(0xffffffffu, nq);
+  if (lane == 0) atomicAdd(&live_quarters, nq);
+  __syncthreads();
   if (threadIdx.x == 0) {
     colcount[rb] = total_live + total_dead;
     colsplit[rb] = total_live;
-    atomicAdd(&sc->visited, (double)(total_live + total_dead));
+    atomicAdd(&sc->visited, 0.25 * (double)live_quarters);  // in whole (row block, column) tiles
   }
 }
 
@@ -1163,7 +1237,8 @@ int launch_sweep1(const spb_em_params* p, const int32_t* bidx, cudaStream_t st) 
   }
   dim3 grid(p->ldx / kRowTile, p->seg1);
   estep_sweep1_kernel<DIM><<<grid, kThreads, sizeof(SmemLayout), st>>>(p->GT, p->ldx, bidx, p->colgeom, p->XAHat, p->lm, p->mm, p->sc,
-                                                                      p->colpart, p->NBb, p->nbb_pad, p->collist, p->colcount, p->colsplit);
+                                                                      p->colpart, p->NBb, p->nbb_pad, p->collist, p->colquarters, p->colcount,
+                                                                      p->colsplit);
   return 0;
 }
 
@@ -1180,7 +1255,8 @@ int launch_sweep2(const spb_em_params* p, const int32_t* bidx, cudaStream_t st) 
   }
   dim3 grid(p->ldx / kRowTile, p->seg2);
   estep_sweep2_kernel<SP, DIM><<<grid, kThreads, sizeof(SmemLayout), st>>>(p->GT, p->ldx, bidx, p->colconst, p->XAHat, p->lm, p->sc,
-                                                                          p->rowpart, p->NBb, p->nbb_pad, p->collist, p->colcount, p->colsplit);
+                                                                          p->rowpart, p->NBb, p->nbb_pad, p->collist, p->colquarters, p->colcount,
+                                                                          p->colsplit);
   return 0;
 }
 
@@ -1218,8 +1294,8 @@ extern "C" int spb_estep_col_lists(const spb_em_params* p, void* stream) {
   }
   const bool all_cols = !(p->svi && p->batch_idx);  // the iteration's columns are the fixed cells themselves, in order
   build_col_lists_kernel<<<nrb, kListThreads, smem, (cudaStream_t)stream>>>(
-      p->bbox, all_cols ? p->xb4 : p->colgeom, all_cols ? 4 : 8, all_cols ? 1 : 2, p->NBb, p->sc, p->cull, p->collist, p->colcount,
-      p->colsplit, p->nbb_pad, colmask, p->keepmask, (p->nbb_pad + 31) / 32);
+      p->bbox, all_cols ? p->xb4 : p->colgeom, all_cols ? 4 : 8, all_cols ? 1 : 2, p->NBb, p->sc, p->cull, p->collist,
+      p->colquarters, p->colcount, p->colsplit, p->nbb_pad, colmask, p->keepmask, (p->nbb_pad + 31) / 32);
   SPB_CHECK_LAUNCH();
   return 0;
 }
