@@ -93,7 +93,9 @@ typedef struct spb_em_params {
   int32_t g_rigid;             /* guidance_effect in ("rigid", "both") */
   int32_t g_NI;                /* number of guidance pairs */
   int32_t sparse_k;            /* > 0: sparse_calculation_mode with sparse_top_k = sparse_k (utils.py:1085-1094) */
-  int32_t NB_total;            /* column-sharded pair: fixed cells of ALL ranks (gamma update); 0 = NBb */
+  int32_t NB_total;            /* columns of the whole iteration when one call sees only a block of them (column-sharded pair: fixed cells of ALL ranks; column chunk: the iteration's NB or batch size); gamma update; 0 = NBb */
+  int32_t gt_by_position;      /* 1: GT row j is the j-th column of THIS call (a cost chunk built for its columns), not fixed cell batch_idx[iter][j] */
+  int32_t fold_add;            /* 1: spb_row_fold adds into rowstat[parity] instead of overwriting it (column chunks of one iteration, folded in order) */
   int32_t reserved1;
   double lambdaVF;
   double gamma_a;
@@ -217,6 +219,10 @@ int spb_gram_prepare(const float* UT, int64_t ldn, int64_t N, int32_t K, const f
 int spb_gram_tc(const float* A_hi, const float* A_lo, const float* B_hi, const float* B_lo, int64_t ldn, int64_t N, int32_t K,
                 int32_t E, const float* mean, const double* sums4, float* scratch, int64_t scratch_floats, double* UtWU,
                 double* UtX, void* stream);
+/* dst[r][0..width) = src[idx[r]][0..width) for r < n, in 4-byte words (pitches in words): the fixed-side operands of the
+   columns of one iteration chunk (tf32 hi / lo, row terms, labels). 16-byte accesses when width, pitches and bases allow. */
+int spb_gather_rows(const void* src, int64_t ld_src, int64_t width, const int32_t* idx, int64_t n, void* dst, int64_t ld_dst,
+                    void* stream);
 /* label layer: GT[j][i] (op)= LT[labA_i][labB_j] */
 int spb_label_cost(const int32_t* labA, const int32_t* labB, const float* LT, int32_t nB_labels, int64_t NA, int64_t NB,
                    int32_t accumulate, float* GT, int64_t ldx, void* stream); /* utils.py:830 */
@@ -233,7 +239,7 @@ int spb_row_finalize(const spb_em_params* p, void* stream);
    rowstat[parity] over the ranks (e.g. ncclAllReduce), finish the row statistics from it; or (2b) ONE kernel that signals
    the peers, waits for their epoch flags and sums their rowstat[parity] straight over NVLink peer memory in rank order
    (bit-identical on every rank) before finishing — no separate collective. epoch must increase by one per call on every rank. */
-int spb_row_fold(const spb_em_params* p, int32_t parity, void* stream);
+int spb_row_fold(const spb_em_params* p, int32_t parity, void* stream); /* p->fold_add: add instead of overwrite */
 int spb_row_stats_finalize(const spb_em_params* p, int32_t parity, void* stream);
 int spb_row_stats_p2p(const spb_em_params* p, int32_t parity, uint64_t epoch, void* stream);
 /* dense P [NA][NBb] (row-major, pitch ldp) of the state left by the last E-step */

@@ -119,6 +119,7 @@ def load_library():
         "spb_rows_normalize": ([P, I64, I64, I64, P, I64, P], C.c_int),
         "spb_split_tf32": ([P, P, P, I64, P], C.c_int),
         "spb_gene_cost_tc": ([P, P, I64, P, P, P, I64, P, I64, I64, I64, I32, I32, F, I32, P, I64, P], C.c_int),
+        "spb_gather_rows": ([P, I64, I64, P, I64, P, I64, P], C.c_int),
         "spb_label_cost": ([P, P, P, I32, I64, I64, I32, P, I64, P], C.c_int),
         "spb_gather_cols": ([EP, I32, P], C.c_int),
         "spb_estep_col_lists": ([EP, P], C.c_int),

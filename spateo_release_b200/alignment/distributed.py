@@ -86,15 +86,34 @@ def morpho_align_chain_sharded(
     return models, transformation
 
 
-def pair_device_bytes(n_moving: int, n_fixed: int, n_genes: int) -> int:
+def pair_device_bytes(n_moving: int, n_fixed: int, n_genes: int, chunk_cols: Optional[int] = None, n_sms: int = 132) -> int:
     """Device memory one prepared pair needs, dominated by its fp32 cost matrix [n_fixed][roundup(n_moving, 512)]; the
     expression operands of the cost precompute (two sides, value + tf32 hi / lo, genes padded to 32) and 1 GiB for the
-    per-cell state are added on top."""
+    per-cell state are added on top.
+
+    ``chunk_cols``: the footprint of a streamed pair instead, whose cost matrix is recomputed every iteration in chunks of
+    that many columns. The resident matrix is replaced by one [chunk_cols][ldx] cost chunk and every per-column buffer of
+    the E-step at that width: column partials, keep masks, work lists, quarter masks, column records, the row partials
+    of the sweep's column segments (``n_sms`` sets their count) and the gathered fixed-side operands of an SVI chunk."""
     from .. import _capi
 
     ldx = -(-n_moving // _capi.ROW_TILE) * _capi.ROW_TILE
     gp = -(-n_genes // 32) * 32
-    return 4 * n_fixed * ldx + 4 * 3 * (n_moving + n_fixed) * gp + (1 << 30)
+    operands = 4 * 3 * (n_moving + n_fixed) * gp + (1 << 30)
+    if chunk_cols is None:
+        return 4 * n_fixed * ldx + operands
+    from .morpho_class import Morpho_pairwise
+
+    nrb = ldx // _capi.ROW_TILE
+    pad = -(-chunk_cols // 8) * 8 + 8
+    per_col = (
+        4 * ldx                                  # cost chunk
+        + nrb * (4 * 4 + 4 + 1) + nrb // 8 + 1   # colpart [nrb][4], collist, colquarters, keepmask bits
+        + 4 + 8 * 4 + _capi.CONST["SPB_COLCONST_FLOATS"] * 4 + _capi.CONST["SPB_COLMASK_WORDS"] * 4  # K_NB, colgeom, colconst, colmask
+        + 2 * 4 * gp + 2 * 4                     # gathered tf32 hi / lo operands, row term, label
+    )
+    seg = Morpho_pairwise._choose_segments(nrb, chunk_cols, n_sms)
+    return pad * per_col + 4 * 8 * ldx * seg + operands
 
 
 def _room_for_next_pair(dev, need: int) -> bool:

@@ -85,6 +85,8 @@ def morpho_align(
     (morpho_alignment.py:22-111). Returns ``(align_models, pis)`` with ``pis[i] = P.T``."""
     aligned = [_working_copy(m) for m in models]
     _seed_keys(aligned, spatial_key, key_added)
+    # the posterior of a pair whose cost matrix is streamed (too large for the device) is not built: its entry of pis is None
+    kwargs.setdefault("materialize_P", "auto")
     pis = []
     for fixed, moving in zip(aligned[:-1], aligned[1:]):
         solver, P = _solve_pair(

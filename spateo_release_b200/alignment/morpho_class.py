@@ -11,7 +11,7 @@ stays on the device, there is no host synchronisation inside the iteration loop 
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Optional, Union
+from typing import List, NamedTuple, Optional, Union
 
 import numpy as np
 import torch
@@ -118,6 +118,83 @@ def kd_order(coords: np.ndarray, tile: int = 512, quarter: int = 128) -> np.ndar
     return np.concatenate([q for b in blocks for q in _kd_groups(c, b, quarter)])
 
 
+def _device_budget(dev) -> int:
+    """Bytes the next allocations on ``dev`` can use: driver-free memory plus what the caching allocator holds unused."""
+    free, _ = torch.cuda.mem_get_info(dev)
+    return free + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+
+
+class CostPlan(NamedTuple):
+    """How a pair holds its expression cost matrix. ``resident``: the whole [N_B][ldx] matrix is built once and kept.
+    ``streamed``: every iteration recomputes it in column chunks ``chunks`` (``[c0, c1)`` ranges over the iteration's
+    ``cols`` columns, ``width`` columns wide except the last) that fit the device next to the rest of the pair."""
+
+    mode: str
+    width: int
+    chunks: tuple
+    need: int
+    budget: int
+
+    @property
+    def streamed(self) -> bool:
+        return self.mode == "streamed"
+
+    @property
+    def n_chunks(self) -> int:
+        return len(self.chunks)
+
+
+def plan_cost(n_moving: int, n_fixed: int, n_genes: int, cols: int, budget: int, n_sms: int = 132) -> CostPlan:
+    """Resident when ``pair_device_bytes`` fits ``budget``; otherwise the widest multiple of 8 columns (at most ``cols``,
+    the columns of one iteration) whose streamed footprint fits, balanced over the chunks it takes. Raises MemoryError
+    when not even 8 columns fit."""
+    from .distributed import pair_device_bytes
+
+    need = pair_device_bytes(n_moving, n_fixed, n_genes)
+    if need <= budget:
+        return CostPlan("resident", cols, ((0, cols),), need, budget)
+
+    def need_at(c):
+        return pair_device_bytes(n_moving, n_fixed, n_genes, chunk_cols=c, n_sms=n_sms)
+
+    if need_at(min(8, cols)) > budget:
+        raise MemoryError(
+            f"the pair ({n_moving} x {n_fixed} cells, {n_genes} features) does not fit the device even with its cost matrix "
+            f"streamed 8 columns at a time: {need_at(min(8, cols))} bytes needed, {budget} bytes available")
+    if need_at(cols) <= budget:
+        width = cols
+    else:
+        lo, hi = 1, (cols - 1) // 8  # 8 lo fits; find the largest multiple of 8 below cols that fits
+        while lo < hi:
+            mid = (lo + hi + 1) // 2
+            if need_at(8 * mid) <= budget:
+                lo = mid
+            else:
+                hi = mid - 1
+        width = 8 * lo
+    n = -(-cols // width)
+    width = min(cols, _round_up(-(-cols // n), 8))  # same chunk count, widths as even as multiples of 8 allow
+    chunks = tuple((c0, min(cols, c0 + width)) for c0 in range(0, cols, width))
+    return CostPlan("streamed", width, chunks, need_at(width), budget)
+
+
+def svi_schedule(batch_perm: np.ndarray, max_iter: int, nbb: int) -> np.ndarray:
+    """[max(max_iter, 1)][nbb] fixed cells of every SVI iteration: a deterministic function of the initial permutation
+    (morpho_class.py:894-896)."""
+    sched = np.empty((max(max_iter, 1), nbb), dtype=np.int32)
+    perm = batch_perm.copy()
+    for it in range(max_iter):
+        sched[it] = perm[:nbb]
+        perm = np.roll(perm, nbb)
+    return sched
+
+
+def svi_chunk_schedules(sched: np.ndarray, chunks) -> list:
+    """Every column chunk's own [max_iter][c1 - c0] slice of the SVI schedule: the chunks of iteration ``it`` together
+    cover the same fixed cells, in the same order, as row ``it`` of ``sched``."""
+    return [np.ascontiguousarray(sched[:, c0:c1]) for c0, c1 in chunks]
+
+
 def resolve_device(device) -> torch.device:
     """Reference semantics: "cpu" or a GPU index string (utils.py:35-66). Here every value maps to a CUDA device —
     there is no CPU path; ``CUDA_VISIBLE_DEVICES`` is NOT mutated (the reference does, utils.py:51)."""
@@ -203,25 +280,37 @@ class GeneCostBuilder:
         return hi, lo
 
     def cost(self, opA, rtA, opB, rtB, NA, NB, G, metric, prob_type, prob_param, accumulate, GT, ldx):
-        pp = float(prob_param) if prob_param is not None else 1.0
         ahi, alo = self._split(opA)
         bhi, blo = self._split(opB)
+        self.cost_split(ahi, alo, rtA, bhi, blo, rtB, NA, NB, G, metric, prob_type, prob_param, accumulate, GT, ldx)
+        self._keep = (ahi, alo, bhi, blo)  # stay alive until the stream has consumed them
+
+    def split_pair(self, opA, rtA, opB, rtB, G):
+        """Operands of ``prepare_pair`` as the tf32 hi / lo pairs ``cost_split`` takes (split once, kept for a streamed run)."""
+        ahi, alo = self._split(opA)
+        bhi, blo = self._split(opB)
+        return dict(ahi=ahi, alo=alo, rtA=rtA, bhi=bhi, blo=blo, rtB=rtB, G=G)
+
+    def cost_split(self, ahi, alo, rtA, bhi, blo, rtB, NA, NB, G, metric, prob_type, prob_param, accumulate, GT, ldx):
+        """GT[j][i] (op)= prob(metric(A_i, B_j)) for the NB rows of the fixed-side operands ``bhi`` / ``blo`` / ``rtB``
+        (all fixed cells, a row range of them or the gathered columns of an iteration chunk)."""
+        pp = float(prob_param) if prob_param is not None else 1.0
         check(
             self.lib.spb_gene_cost_tc(
-                ptr(ahi), ptr(alo), opA.stride(0), ptr(rtA), ptr(bhi), ptr(blo), opB.stride(0), ptr(rtB), NA, NB, G,
+                ptr(ahi), ptr(alo), ahi.stride(0), ptr(rtA), ptr(bhi), ptr(blo), bhi.stride(0), ptr(rtB), NA, NB, G,
                 _METRIC_CODE[metric], _PROB_CODE[prob_type], pp, 1 if accumulate else 0, ptr(GT), ldx,
                 _capi.current_stream_ptr(),
             ),
             "spb_gene_cost_tc",
         )
-        self._keep = (ahi, alo, bhi, blo)  # stay alive until the stream has consumed them
 
 
 class Morpho_pairwise:
     """Align a moving slice ``sampleA`` onto a fixed slice ``sampleB`` (same constructor as morpho_class.py:110-167).
 
     Extra keywords (not in the reference): ``materialize_P`` — when False ``run()`` skips building the dense
-    N_A x N_B posterior (40 GB at 100k x 100k) and returns None; every other output is unaffected.
+    N_A x N_B posterior (40 GB at 100k x 100k) and returns None; every other output is unaffected; ``"auto"`` builds it
+    unless the cost matrix is streamed (the default of ``morpho_align``).
     ``compute_mapping`` — ``self.mapping`` (an ``ArgmaxPi``) receives the row / column maxima of the final posterior from a
     fused kernel, for ``get_optimal_mapping_relationship`` / ``mapping_aligned_coords`` without a dense P.
     ``spatial_sort`` / ``cull_zero_tiles`` — the moving cells are processed in k-d order (``kd_order``) so that each row block
@@ -229,6 +318,13 @@ class Morpho_pairwise:
     of rows whose every pair underflows to exactly 0 in fp32 are neither read nor computed; results are bit-identical to the
     dense sweep in the same row order (all outputs are returned in the caller's row order).
     ``column_shard`` — set by ``morpho_align_pair_sharded``: one pair's fixed cells split over several GPUs.
+    Cost matrix: resident ([N_B][roundup(N_A, 512)] fp32, built once) whenever the pair fits the device's free memory,
+    otherwise streamed — recomputed every iteration in column chunks that fit (``cost_plan`` records which, the chunk width
+    and count; ``verbose`` prints it). This is chosen from the input size and the device alone, and lets one GPU align pairs
+    above ~135k cells per slice (80 GB). A streamed pair supports full EM and SVI, every metric, multi-layer products, guidance,
+    ``kernel_type="geodist"``, any K, ``sparse_calculation_mode``, ``return_mapping`` and ``iter_key_added``; it refuses
+    (NotImplementedError) dense ``materialize_P=True``, ``compute_mapping`` and ``column_shard``. With one chunk (default SVI)
+    its results are bit-identical to the resident run.
     Accepted but without effect (memory work-arounds whose results are identical): ``use_chunk``, ``chunk_capacity``,
     ``pre_compute_dist``. ``sparse_calculation_mode`` keeps the top ``sparse_top_k`` posterior entries of every column by an
     exact on-device radix select (P comes back as ``scipy.sparse.coo_matrix``). Not implemented (NotImplementedError):
@@ -408,7 +504,7 @@ class Morpho_pairwise:
                 )
         # ---- features of the reference that this round does not cover: fail loudly, never silently differ ----
         if self.sparse_calculation_mode:
-            self.pre_compute_dist = False  # morpho_class.py:439-440 (no effect here: the cost matrix is always resident)
+            self.pre_compute_dist = False  # morpho_class.py:439-440 (no effect here: residency follows the pair's size)
             if int(self.sparse_top_k) < 1:
                 raise ValueError("sparse_top_k must be a positive integer.")
         if self.kernel_type not in ("euc", "geodist"):
@@ -805,6 +901,10 @@ class Morpho_pairwise:
         self._set_row_order()
         c0, c1 = self._col_range()
         nb_loc = c1 - c0
+        self._plan_cost(nb_loc)
+        if self.cost_plan.streamed:
+            self._prepare_streamed_cost()
+            return
         self._GT = torch.empty((nb_loc, self.ldx), dtype=torch.float32, device=dev)
         gc = GeneCostBuilder(lib, dev)
         first = True
@@ -830,6 +930,122 @@ class Morpho_pairwise:
                 del A, B, opA, opB
             first = False
         self.__dict__.pop("_dev_rep", None)  # the resident copies of the representations are no longer needed
+
+    def _cost_features(self) -> int:
+        """Features of the expression operands of all layers together (sym_kl contracts over both of its halves)."""
+        return sum(0 if d == "label" else (2 * _round_up(e.shape[1], 32) if d == "sym_kl" else e.shape[1])
+                   for e, d in zip(self.exp_layers_A, self.dissimilarity))
+
+    def _plan_cost(self, nb_loc: int):
+        """Resident or streamed cost matrix, from the pair's size and the memory the device has (``plan_cost``)."""
+        cols = min(self.batch_size, nb_loc) if self.SVI_mode else nb_loc
+        n_sms = torch.cuda.get_device_properties(self._dev).multi_processor_count
+        plan = plan_cost(self.NA, nb_loc, self._cost_features(), cols, _device_budget(self._dev), n_sms)
+        if isinstance(self.materialize_P, str) and self.materialize_P == "auto":  # the public drivers' default
+            self.materialize_P = not plan.streamed
+        if plan.streamed:
+            why = None
+            if self.column_shard is not None:
+                why = "column_shard: a column-sharded pair keeps its block of the cost matrix resident"
+            elif self.compute_mapping:
+                why = "compute_mapping: the posterior maxima are read from the resident cost matrix after the run"
+            elif self.materialize_P and not self.sparse_calculation_mode:
+                why = "materialize_P=True: a dense P is as large as the cost matrix that does not fit"
+            if why is not None:
+                raise NotImplementedError(
+                    f"the cost matrix of this pair ({plan.need} bytes streamed, {plan.budget} available) does not fit the "
+                    f"device and is streamed in column chunks, which does not support {why}")
+        self.cost_plan = plan
+        if self.verbose:
+            if plan.streamed:
+                print(f"|-----> Cost matrix streamed: {plan.n_chunks} chunk(s) of {plan.width} columns per iteration "
+                      f"({plan.need / 2**30:.1f} GiB of {plan.budget / 2**30:.1f} GiB).")
+            else:
+                print(f"|-----> Cost matrix resident ({plan.need / 2**30:.1f} GiB of {plan.budget / 2**30:.1f} GiB).")
+
+    @property
+    def _streamed(self) -> bool:
+        plan = getattr(self, "cost_plan", None)
+        return plan is not None and plan.streamed
+
+    def _prepare_streamed_cost(self):
+        """Streamed cost matrix: the operands of every layer, split into tf32 hi / lo once and kept for the run, and one
+        [width][ldx] chunk that every iteration refills column chunk by column chunk (``_chunk_cost``)."""
+        dev, lib = self._dev, self._lib
+        width = self.cost_plan.width
+        gc = GeneCostBuilder(lib, dev)
+        self._gc, self._layers = gc, []
+        for eA, eB, d_s, p_t, p_p in zip(
+            self.exp_layers_A, self.exp_layers_B, self.dissimilarity, self.probability_type, self.probability_parameters
+        ):
+            if d_s == "label":
+                L = dict(
+                    kind="label",
+                    la=torch.from_numpy(np.ascontiguousarray(eA if self._perm is None else eA[self._perm], dtype=np.int32)).to(dev),
+                    lb=torch.from_numpy(np.ascontiguousarray(eB, dtype=np.int32)).to(dev),
+                    LT=torch.from_numpy(np.ascontiguousarray(self.label_transfer, dtype=np.float32)).to(dev),
+                )
+                if self.SVI_mode:
+                    L["lb_g"] = torch.empty((width,), dtype=torch.int32, device=dev)
+            else:
+                A = self._to_device_pinned(eA)
+                if self._perm is not None:
+                    A = A.index_select(0, self._perm_dev)
+                B = self._to_device_pinned(eB)
+                L = gc.split_pair(*gc.prepare_pair(A, B, d_s))
+                del A, B
+                L.update(kind="tc", metric=d_s, p_t=p_t, p_p=p_p)
+                if self.SVI_mode:
+                    L["g"] = dict(bhi=torch.empty((width, L["bhi"].shape[1]), dtype=torch.float32, device=dev),
+                                  blo=torch.empty((width, L["blo"].shape[1]), dtype=torch.float32, device=dev),
+                                  rtB=None if L["rtB"] is None else torch.empty((width,), dtype=torch.float32, device=dev))
+            self._layers.append(L)
+        self.__dict__.pop("_dev_rep", None)
+        self._GT = torch.empty((width, self.ldx), dtype=torch.float32, device=dev)
+        self.cost_events = None  # a list: (start, end) CUDA events around the cost of every chunk are appended to it
+
+    def _gather(self, src: torch.Tensor, idx: torch.Tensor, n: int, dst: torch.Tensor):
+        """dst[:n] = src[idx[:n]] (rows of 4-byte words) on the device."""
+        width = src.shape[1] if src.dim() == 2 else 1
+        ld_src = src.stride(0) if src.dim() == 2 else 1
+        ld_dst = dst.stride(0) if dst.dim() == 2 else 1
+        check(self._lib.spb_gather_rows(ptr(src), ld_src, width, ptr(idx), n, ptr(dst), ld_dst, _capi.current_stream_ptr()),
+              "spb_gather_rows")
+
+    def _chunk_cost(self, c0: int, c1: int, idx: Optional[torch.Tensor]):
+        """Cost rows of one column chunk into ``_GT`` (row j = column c0 + j of the iteration): the fixed cells [c0, c1)
+        when ``idx`` is None, else the fixed cells ``idx`` (this iteration's row of the chunk's SVI schedule), whose
+        operands are gathered first."""
+        lib, NA, ldx, st = self._lib, self.NA, self.ldx, _capi.current_stream_ptr()
+        n = c1 - c0
+        ev = self.cost_events
+        if ev is not None:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        for k, L in enumerate(self._layers):
+            if L["kind"] == "label":
+                lb = L["lb"][c0:c1]
+                if idx is not None:
+                    self._gather(L["lb"], idx, n, L["lb_g"])
+                    lb = L["lb_g"]
+                check(lib.spb_label_cost(ptr(L["la"]), ptr(lb), ptr(L["LT"]), L["LT"].shape[1], NA, n, 1 if k else 0,
+                                         ptr(self._GT), ldx, st), "spb_label_cost")
+                continue
+            if idx is None:
+                bhi, blo = L["bhi"][c0:c1], L["blo"][c0:c1]
+                rtB = None if L["rtB"] is None else L["rtB"][c0:c1]
+            else:
+                g = L["g"]
+                self._gather(L["bhi"], idx, n, g["bhi"])
+                self._gather(L["blo"], idx, n, g["blo"])
+                if g["rtB"] is not None:
+                    self._gather(L["rtB"], idx, n, g["rtB"])
+                bhi, blo, rtB = g["bhi"], g["blo"], g["rtB"]
+            self._gc.cost_split(L["ahi"], L["alo"], L["rtA"], bhi, blo, rtB, NA, n, L["G"], L["metric"], L["p_t"], L["p_p"],
+                                k > 0, self._GT, ldx)
+        if ev is not None:
+            e1.record()
+            ev.append((e0, e1))
 
     def _col_range(self):
         """Fixed cells (columns of P) held by this process: all of them, or this rank's block of a column-sharded pair."""
@@ -903,7 +1119,9 @@ class Morpho_pairwise:
         nbb_alloc = NB if (self.return_mapping and self.SVI_mode) else nbb
         self._NBb = nbb
         nrb = ldx // _capi.ROW_TILE
-        self._nbb_pad = _round_up(nbb_alloc, 8) + 8
+        # per-column buffers hold every column of an E-step, or one column chunk of it when the cost matrix is streamed
+        width = self.cost_plan.width if self._streamed else nbb_alloc
+        self._nbb_pad = _round_up(width, 8) + 8
         s = {}
         s["xa"] = torch.zeros((3, ldx), dtype=f32, device=dev)
         s["xa"][:D, :NA] = torch.from_numpy(np.ascontiguousarray(self._sorted(self.coordsA).T, dtype=np.float32)).to(dev)
@@ -928,15 +1146,15 @@ class Morpho_pairwise:
             s[k] = torch.zeros((ldx,), dtype=f32, device=dev)
         s["PXB"] = torch.zeros((3, ldx), dtype=f32, device=dev)
         s["PXB_term"] = torch.zeros((3, ldx), dtype=f32, device=dev)
-        s["K_NB"] = torch.zeros((self._nbb_pad,), dtype=f32, device=dev)
+        s["K_NB"] = torch.zeros((_round_up(nbb_alloc, 8) + 8,), dtype=f32, device=dev)
         s["colgeom"] = torch.zeros((self._nbb_pad, 8), dtype=f32, device=dev)
         s["colconst"] = torch.zeros((self._nbb_pad, _capi.CONST["SPB_COLCONST_FLOATS"]), dtype=f32, device=dev)
         s["colpart"] = torch.zeros((nrb, 4, self._nbb_pad), dtype=f32, device=dev)
         s["keepmask"] = torch.zeros((nrb, (self._nbb_pad + 31) // 32), dtype=torch.int32, device=dev)
         n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
-        seg1 = self._choose_segments(nrb, nbb, n_sms)
-        seg2 = self._choose_segments(nrb, nbb, n_sms)
-        seg_alloc = max(seg2, self._choose_segments(nrb, nbb_alloc, n_sms))
+        seg1 = self._choose_segments(nrb, min(nbb, width), n_sms)
+        seg2 = self._choose_segments(nrb, min(nbb, width), n_sms)
+        seg_alloc = max(seg2, self._choose_segments(nrb, width, n_sms))
         s["rowpart"] = torch.zeros((seg_alloc, 8, ldx), dtype=f32, device=dev)
         s["bbox"] = torch.zeros((nrb, 4, 8), dtype=f32, device=dev)
         s["collist"] = torch.zeros((nrb, self._nbb_pad), dtype=torch.int32, device=dev)
@@ -954,16 +1172,15 @@ class Morpho_pairwise:
         s["trace_buf"] = torch.zeros((max(self.max_iter, 1), _capi.TRACE_STRIDE), dtype=f64, device=dev)
         s["optimal"] = torch.zeros((12,), dtype=f64, device=dev)
         if self.SVI_mode:
-            # the whole batch schedule is a deterministic function of the initial permutation (morpho_class.py:894-896)
-            sched = np.empty((max(self.max_iter, 1), nbb), dtype=np.int32)
-            perm = self.batch_perm.copy()
-            for it in range(self.max_iter):
-                sched[it] = perm[:nbb]
-                perm = np.roll(perm, nbb)
+            sched = svi_schedule(self.batch_perm, self.max_iter, nbb)
             self.batch_idx = sched[self.max_iter - 1].astype(np.int64) if self.max_iter > 0 else None
             s["batch_idx"] = torch.from_numpy(sched).to(dev)
+            if self._streamed:
+                s["chunk_sched"] = [torch.from_numpy(q).to(dev) for q in svi_chunk_schedules(sched, self.cost_plan.chunks)]
         else:
             s["batch_idx"] = None
+        if self._streamed:  # fp64 row statistics, summed over the column chunks of an E-step (spb_row_fold)
+            s["rowstat"] = torch.zeros((2 * 8 * ldx,), dtype=f64, device=dev)
         # scalars
         sc = SpbScalars()
         sc.sigma2 = float(self._sigma2_init)
@@ -989,6 +1206,8 @@ class Morpho_pairwise:
         p.rowstat = p.peer_rowstat = p.shard_flags = p.peer_flags = None
         if self.column_shard is not None:
             self._setup_column_shard(p, s)
+        if self._streamed:
+            p.rowstat = s["rowstat"].data_ptr()
         p.svi, p.nn_init, p.update_R = int(self.SVI_mode), int(self.nn_init), int(self.update_R)
         p.nonrigid_start_iter = int(self.nonrigid_start_iter)
         p.seg1, p.seg2, p.nbb_pad, p.trace = seg1, seg2, self._nbb_pad, 1
@@ -1177,12 +1396,15 @@ class Morpho_pairwise:
         lib, p = self._lib, self._params
         nonrigid = it > self.nonrigid_start_iter
         large_K = nonrigid and self.K > _capi.MAX_K_FUSED
-        if not (large_K or capture_P or sweep_events is not None or self.column_shard is not None):
+        if not (large_K or capture_P or sweep_events is not None or self.column_shard is not None or self._streamed):
             check(lib.spb_em_iteration(C.byref(p), it, st), "spb_em_iteration")
             return
-        self._estep_only(it, st, sweep_events)
-        if capture_P:
-            self._capture_P(it, st)
+        if self._streamed:
+            self._estep_only(it, st, on_chunk=self._streamed_capture() if capture_P else None)
+        else:
+            self._estep_only(it, st, sweep_events)
+            if capture_P:
+                self._capture_P(it, st)
         check(lib.spb_update_gamma_alpha(C.byref(p), st), "spb_update_gamma_alpha")
         if nonrigid:
             check(lib.spb_nonrigid_accumulate(C.byref(p), st), "spb_nonrigid_accumulate")
@@ -1232,9 +1454,12 @@ class Morpho_pairwise:
         return sp.coo_matrix((vals.cpu().numpy().astype(dt).reshape(-1), (rows.reshape(-1), col)),
                              shape=(self.NA, self._NBb))
 
-    def _estep_only(self, it: int, st, sweep_events: Optional[list] = None):
+    def _estep_only(self, it: int, st, sweep_events: Optional[list] = None, on_chunk=None):
         """One E-step + the statistics the closing similarity needs (used for return_mapping under SVI)."""
         lib, p = self._lib, self._params
+        if self._streamed:
+            self._estep_streamed(it, st, on_chunk)
+            return
         check(lib.spb_iter_begin(C.byref(p), it, st), "spb_iter_begin")
         check(lib.spb_gather_cols(C.byref(p), it, st), "spb_gather_cols")
         check(lib.spb_estep_col_lists(C.byref(p), st), "spb_estep_col_lists")
@@ -1257,6 +1482,68 @@ class Morpho_pairwise:
             self._shard_row_statistics(st)
         else:
             check(lib.spb_row_finalize(C.byref(p), st), "spb_row_finalize")
+
+    def _chunk_params(self, k: int, c0: int, c1: int) -> SpbEmParams:
+        """Parameters of one column chunk [c0, c1) of the E-step that ``_params`` describes: its columns are fixed cells
+        [c0, c1) (full EM, or the full posterior of return_mapping) or positions [c0, c1) of the SVI batch, whose schedule
+        is the chunk's own slice; the cost chunk holds them by position, the column sums land in K_NB[c0:c1]."""
+        p, s = self._params, self._state
+        q = SpbEmParams.from_buffer_copy(p)
+        q.NBb, q.NB_total, q.gt_by_position = c1 - c0, p.NBb, 1
+        q.GT = self._GT.data_ptr()
+        q.K_NB = s["K_NB"].data_ptr() + 4 * c0
+        if p.svi:
+            q.batch_idx = s["chunk_sched"][k].data_ptr()
+        else:
+            q.batch_idx = None
+            q.xb4 = s["xb4"].data_ptr() + 16 * c0
+        return q
+
+    def _estep_streamed(self, it: int, st, on_chunk=None):
+        """One E-step with the cost matrix recomputed chunk by chunk: per chunk the cost rows, then the E-step pieces up to
+        sweep 2, whose row partials are folded into the fp64 row statistics in chunk order (reproducible); the statistics are
+        finished once. ``on_chunk(params, it, c0, c1)`` runs after a chunk's sweep 2, while its cost rows and column constants
+        are live."""
+        lib, p, s = self._lib, self._params, self._state
+        check(lib.spb_iter_begin(C.byref(p), it, st), "spb_iter_begin")
+        cols, width = p.NBb, self.cost_plan.width
+        for k, c0 in enumerate(range(0, cols, width)):
+            c1 = min(cols, c0 + width)
+            q = self._chunk_params(k, c0, c1)
+            q.fold_add = int(k > 0)
+            self._chunk_cost(c0, c1, s["chunk_sched"][k][it] if p.svi else None)
+            if c1 - c0 < width:  # ragged chunk: the pad column record after the last column is zero, as in a full one
+                s["colgeom"][c1 - c0:].zero_()
+                s["colconst"][c1 - c0:].zero_()
+            qp = C.byref(q)
+            check(lib.spb_gather_cols(qp, it, st), "spb_gather_cols")
+            check(lib.spb_estep_col_lists(qp, st), "spb_estep_col_lists")
+            check(lib.spb_estep_sweep1(qp, it, st), "spb_estep_sweep1")
+            check(lib.spb_col_finalize(qp, st), "spb_col_finalize")
+            if self.sparse_calculation_mode:
+                check(lib.spb_estep_col_select(qp, it, st), "spb_estep_col_select")
+            check(lib.spb_estep_sweep2(qp, it, st), "spb_estep_sweep2")
+            if on_chunk is not None:
+                on_chunk(q, it, c0, c1)
+            check(lib.spb_row_fold(qp, 0, st), "spb_row_fold")
+        check(lib.spb_row_stats_finalize(C.byref(p), 0, st), "spb_row_stats_finalize")
+
+    def _streamed_capture(self):
+        """Posterior capture of a streamed E-step (sparse mode only: the COO entries of every chunk's columns, emitted while
+        the chunk is live); None when nothing is captured."""
+        if not (self.materialize_P and self.sparse_calculation_mode):
+            self._P_dev = "skipped"
+            return None
+        k = int(self.sparse_top_k)
+        self._P_rows = torch.zeros((self._NBb, k), dtype=torch.int32, device=self._dev)
+        self._P_vals = torch.zeros((self._NBb, k), dtype=torch.float32, device=self._dev)
+        self._P_dev = "sparse"
+
+        def emit(q, it, c0, c1):
+            check(self._lib.spb_sparse_P_emit(C.byref(q), it, ptr(self._P_rows[c0:c1]), ptr(self._P_vals[c0:c1]),
+                                              _capi.current_stream_ptr()), "spb_sparse_P_emit")
+
+        return emit
 
     def prepare_host(self):
         """Coarse rigid initialisation + variational initialisation (host numpy with small device helpers); consumes
@@ -1319,7 +1606,7 @@ class Morpho_pairwise:
                 want_P = (self.materialize_P or self.compute_mapping) and last and not (self.return_mapping and self.SVI_mode)
                 nonrigid = it > self.nonrigid_start_iter
                 plain = (hist is not None or sweep_events is not None or want_P or self.column_shard is not None
-                         or (nonrigid and self.K > _capi.MAX_K_FUSED))
+                         or self._streamed or (nonrigid and self.K > _capi.MAX_K_FUSED))
                 if not plain:
                     # iterations [it, stop) share the phase and need nothing from the host
                     stop = min(end, self.nonrigid_start_iter + 1) if not nonrigid else end
@@ -1408,17 +1695,23 @@ class Morpho_pairwise:
             sc.sigma2 = float(self.sigma2_end)
             s["sc"].copy_(torch.from_numpy(np.frombuffer(bytes(sc), dtype=np.uint8).copy()))
             check(lib.spb_row_update(C.byref(p), st), "spb_row_update")
+        full_mapping = self.return_mapping and self.SVI_mode
+
+        def capture():  # a streamed E-step captures the posterior while its chunks are live
+            return self._streamed_capture() if self._streamed and getattr(self, "_P_dev", None) is None else None
+
         if self.max_iter == 0:
-            self._estep_only(0, st)
+            self._estep_only(0, st, on_chunk=None if full_mapping else capture())
             check(lib.spb_rigid_moments(C.byref(p), st), "spb_rigid_moments")
-        if self.return_mapping and self.SVI_mode:
+        if full_mapping:
             # full (non-SVI) posterior with the final parameters (morpho_class.py:300-302)
             self.SVI_mode = False
             p.svi, p.NBb = 0, self.NB
-            p.seg1 = p.seg2 = self._choose_segments(self.ldx // _capi.ROW_TILE, self.NB,
-                                                    torch.cuda.get_device_properties(self._dev).multi_processor_count)
+            if not self._streamed:  # streamed: the column segments stay those of the chunk width
+                p.seg1 = p.seg2 = self._choose_segments(self.ldx // _capi.ROW_TILE, self.NB,
+                                                        torch.cuda.get_device_properties(self._dev).multi_processor_count)
             self._NBb = self.NB
-            self._estep_only(last_iter, st)
+            self._estep_only(last_iter, st, on_chunk=capture())
             # scalar Sp's must become the un-averaged sums (morpho_class.py:1183-1185)
             sc = self._read_scalars()
             sc.Sp_spatial, sc.Sp_sigma2, sc.Sp = sc.sums[0], sc.sums[1], sc.sums[2]

@@ -582,7 +582,7 @@ row_finalize_kernel(const float* __restrict__ rowpart, int nseg, int ldx, int NA
 
 // ---- column-sharded pair ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-row_fold_kernel(const float* __restrict__ rowpart, int nseg, int ldx, int NA, double* __restrict__ out) {
+row_fold_kernel(const float* __restrict__ rowpart, int nseg, int ldx, int NA, int add, double* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= NA) return;
   double a[7] = {0, 0, 0, 0, 0, 0, 0};
@@ -591,7 +591,7 @@ row_fold_kernel(const float* __restrict__ rowpart, int nseg, int ldx, int NA, do
     for (int q = 0; q < 7; ++q) a[q] += (double)rowpart[((int64_t)s * 8 + q) * ldx + i];
   }
 #pragma unroll
-  for (int q = 0; q < 7; ++q) out[(int64_t)q * ldx + i] = a[q];
+  for (int q = 0; q < 7; ++q) out[(int64_t)q * ldx + i] = add ? out[(int64_t)q * ldx + i] + a[q] : a[q];
 }
 
 __global__ void __launch_bounds__(256)
@@ -1266,6 +1266,10 @@ int launch_sweep2(const spb_em_params* p, const int32_t* bidx, cudaStream_t st) 
 static inline const int32_t* batch_ptr(const spb_em_params* p, int /*iter*/) {
   return (p->svi && p->batch_idx) ? p->batch_idx : nullptr;
 }
+// schedule the GT readers index their rows by: none when GT holds this call's columns in list order (p->gt_by_position)
+static inline const int32_t* gt_batch_ptr(const spb_em_params* p, int iter) {
+  return p->gt_by_position ? nullptr : batch_ptr(p, iter);
+}
 
 extern "C" int spb_gather_cols(const spb_em_params* p, int32_t iter, void* stream) {
   gather_cols_kernel<<<(p->NBb + 255) / 256, 256, 0, (cudaStream_t)stream>>>(p->xb4, batch_ptr(p, iter), p->sc, p->NBb, p->colgeom);
@@ -1303,8 +1307,8 @@ extern "C" int spb_estep_col_lists(const spb_em_params* p, void* stream) {
 extern "C" int spb_estep_sweep1(const spb_em_params* p, int32_t iter, void* stream) {
   int rc;
   // writes the partial column sums of every (row block, listed column) combination; col_finalize reads exactly those (keepmask)
-  if (p->D == 2) rc = launch_sweep1<2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else rc = launch_sweep1<>(p, batch_ptr(p, iter), (cudaStream_t)stream);
+  if (p->D == 2) rc = launch_sweep1<2>(p, gt_batch_ptr(p, iter), (cudaStream_t)stream);
+  else rc = launch_sweep1<>(p, gt_batch_ptr(p, iter), (cudaStream_t)stream);
   if (rc) return rc;
   SPB_CHECK_LAUNCH();
   return 0;
@@ -1319,10 +1323,10 @@ extern "C" int spb_col_finalize(const spb_em_params* p, void* stream) {
 
 extern "C" int spb_estep_sweep2(const spb_em_params* p, int32_t iter, void* stream) {
   int rc;
-  if (p->sparse_k > 0 && p->D == 2) rc = launch_sweep2<true, 2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else if (p->sparse_k > 0) rc = launch_sweep2<true>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else if (p->D == 2) rc = launch_sweep2<false, 2>(p, batch_ptr(p, iter), (cudaStream_t)stream);
-  else rc = launch_sweep2<false>(p, batch_ptr(p, iter), (cudaStream_t)stream);
+  if (p->sparse_k > 0 && p->D == 2) rc = launch_sweep2<true, 2>(p, gt_batch_ptr(p, iter), (cudaStream_t)stream);
+  else if (p->sparse_k > 0) rc = launch_sweep2<true>(p, gt_batch_ptr(p, iter), (cudaStream_t)stream);
+  else if (p->D == 2) rc = launch_sweep2<false, 2>(p, gt_batch_ptr(p, iter), (cudaStream_t)stream);
+  else rc = launch_sweep2<false>(p, gt_batch_ptr(p, iter), (cudaStream_t)stream);
   if (rc) return rc;
   SPB_CHECK_LAUNCH();
   return 0;
@@ -1339,7 +1343,7 @@ extern "C" int spb_estep_col_select(const spb_em_params* p, int32_t iter, void* 
     if (e != cudaSuccess) return (int)e;
     attr_set[dev_] = true;
   }
-  col_select_kernel<<<p->NBb, kSelThreads, smem, (cudaStream_t)stream>>>(p->GT, p->ldx, batch_ptr(p, iter), p->colconst,
+  col_select_kernel<<<p->NBb, kSelThreads, smem, (cudaStream_t)stream>>>(p->GT, p->ldx, gt_batch_ptr(p, iter), p->colconst,
                                                                       p->XAHat, p->lm, p->sc, p->NA, p->sparse_k, p->K_NB,
                                                                       (p->cull && p->ldx / kRowTile <= 32 * SPB_COLMASK_WORDS) ? p->colmask : nullptr);
   SPB_CHECK_LAUNCH();
@@ -1348,7 +1352,7 @@ extern "C" int spb_estep_col_select(const spb_em_params* p, int32_t iter, void* 
 
 extern "C" int spb_sparse_P_emit(const spb_em_params* p, int32_t iter, int32_t* rows, float* vals, void* stream) {
   if (p->sparse_k <= 0) return SPB_EINVAL;
-  col_emit_kernel<<<p->NBb, kSelThreads, 0, (cudaStream_t)stream>>>(p->GT, p->ldx, batch_ptr(p, iter), p->colconst, p->XAHat,
+  col_emit_kernel<<<p->NBb, kSelThreads, 0, (cudaStream_t)stream>>>(p->GT, p->ldx, gt_batch_ptr(p, iter), p->colconst, p->XAHat,
                                                                     p->lm, p->sc, p->NA, p->sparse_k, rows, vals);
   SPB_CHECK_LAUNCH();
   return 0;
@@ -1358,7 +1362,7 @@ extern "C" int spb_posterior_argmax(const spb_em_params* p, int32_t iter, uint64
                                     void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (colbest) {
-    col_argmax_kernel<<<p->NBb, kSelThreads, 0, st>>>(p->GT, p->ldx, batch_ptr(p, iter), p->colconst, p->XAHat, p->lm,
+    col_argmax_kernel<<<p->NBb, kSelThreads, 0, st>>>(p->GT, p->ldx, gt_batch_ptr(p, iter), p->colconst, p->XAHat, p->lm,
                                                       p->sc, p->NA, (unsigned long long*)colbest);
     SPB_CHECK_LAUNCH();
   }
@@ -1368,7 +1372,7 @@ extern "C" int spb_posterior_argmax(const spb_em_params* p, int32_t iter, uint64
     const int nrow = (p->NA + 255) / 256;
     int nseg = (spb_num_sms() * 8 + nrow - 1) / nrow;  // ~8 CTAs per SM
     nseg = nseg < 1 ? 1 : (nseg > p->NBb ? p->NBb : nseg);
-    row_argmax_kernel<<<dim3(nrow, nseg), 256, 0, st>>>(p->GT, p->ldx, batch_ptr(p, iter), p->colconst, p->XAHat, p->lm,
+    row_argmax_kernel<<<dim3(nrow, nseg), 256, 0, st>>>(p->GT, p->ldx, gt_batch_ptr(p, iter), p->colconst, p->XAHat, p->lm,
                                                         p->sc, p->NA, p->NBb, (unsigned long long*)rowbest);
     SPB_CHECK_LAUNCH();
   }
@@ -1387,7 +1391,7 @@ extern "C" int spb_row_finalize(const spb_em_params* p, void* stream) {
 
 extern "C" int spb_row_fold(const spb_em_params* p, int32_t parity, void* stream) {
   if (p->rowstat == nullptr) return SPB_EINVAL;
-  row_fold_kernel<<<(p->NA + 255) / 256, 256, 0, (cudaStream_t)stream>>>(p->rowpart, p->seg2, p->ldx, p->NA,
+  row_fold_kernel<<<(p->NA + 255) / 256, 256, 0, (cudaStream_t)stream>>>(p->rowpart, p->seg2, p->ldx, p->NA, p->fold_add,
                                                                           p->rowstat + (int64_t)(parity & 1) * 8 * p->ldx);
   SPB_CHECK_LAUNCH();
   return 0;
@@ -1415,7 +1419,7 @@ extern "C" int spb_row_stats_p2p(const spb_em_params* p, int32_t parity, uint64_
 
 extern "C" int spb_materialize_P(const spb_em_params* p, int32_t iter, float* P, int64_t ldp, void* stream) {
   dim3 grid((p->NA + 31) / 32, (p->NBb + 31) / 32), block(32, 8);
-  materialize_P_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(p->GT, p->ldx, batch_ptr(p, iter), p->colconst, p->XAHat,
+  materialize_P_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(p->GT, p->ldx, gt_batch_ptr(p, iter), p->colconst, p->XAHat,
                                                                 p->lm, p->sc, p->NA, p->NBb, P, ldp);
   SPB_CHECK_LAUNCH();
   return 0;

@@ -172,6 +172,24 @@ __global__ void split_tf32_kernel(const float* __restrict__ x, float* __restrict
   }
 }
 
+// dst[r][.] = src[idx[r]][.]: one thread per (row, 16-byte vector) with kVec, per (row, word) otherwise
+template <bool kVec>
+__global__ void __launch_bounds__(256)
+gather_rows_kernel(const uint32_t* __restrict__ src, int64_t ld_src, int64_t width, const int32_t* __restrict__ idx, int64_t n,
+                   uint32_t* __restrict__ dst, int64_t ld_dst) {
+  const int64_t per = kVec ? width / 4 : width;
+  const int64_t total = n * per;
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = t / per, c = t - r * per;
+    const int64_t s = (int64_t)__ldg(idx + r);
+    if constexpr (kVec) {
+      reinterpret_cast<uint4*>(dst + r * ld_dst)[c] = __ldg(reinterpret_cast<const uint4*>(src + s * ld_src) + c);
+    } else {
+      dst[r * ld_dst + c] = __ldg(src + s * ld_src + c);
+    }
+  }
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -241,6 +259,22 @@ extern "C" int spb_gene_cost_tc(const float* A_hi, const float* A_lo, int64_t ld
   gene_cost_tc_kernel<<<grid, kTcThreads, sizeof(TcSmem) + 1024, ST>>>(ma_hi, ma_lo, mb_hi, mb_lo, rowtermA, rowtermB, NA, NB,
                                                                         (int)(Gp / TK), tiles_i, tiles_j, metric, prob_type,
                                                                         neg_inv2b, accumulate, GT, ldx);
+  SPB_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int spb_gather_rows(const void* src, int64_t ld_src, int64_t width, const int32_t* idx, int64_t n, void* dst,
+                               int64_t ld_dst, void* stream) {
+  if (n < 0 || width < 0 || ld_src < width || ld_dst < width) return SPB_EINVAL;
+  if (n == 0 || width == 0) return 0;
+  const bool vec = width % 4 == 0 && ld_src % 4 == 0 && ld_dst % 4 == 0 && ((uintptr_t)src & 15) == 0 &&
+                   ((uintptr_t)dst & 15) == 0;
+  const int64_t work = n * (vec ? width / 4 : width);
+  const int blocks = (int)std::min<int64_t>((work + 255) / 256, (int64_t)spb_num_sms() * 16);
+  const uint32_t* s = static_cast<const uint32_t*>(src);
+  uint32_t* d = static_cast<uint32_t*>(dst);
+  if (vec) gather_rows_kernel<true><<<blocks, 256, 0, ST>>>(s, ld_src, width, idx, n, d, ld_dst);
+  else gather_rows_kernel<false><<<blocks, 256, 0, ST>>>(s, ld_src, width, idx, n, d, ld_dst);
   SPB_CHECK_LAUNCH();
   return 0;
 }
