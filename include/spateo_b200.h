@@ -64,7 +64,7 @@ typedef struct spb_scalars {
   double t[3];           /* (:1398-1402) */
   double dotKS;          /* sum_i K_NA_sigma2_i * SigmaDiag_i (:1427) */
   double sums[8];        /* scratch: Sp_spatial_new, Sp_sigma2_new, Sp_new, S2 */
-  double visited;        /* (row block, column) tiles read by this iteration's sweeps, a tile counting (live 128-row quarters) / 4 (all of them without culling) */
+  double visited;        /* (row block, column) tiles read by this iteration's sweeps, a tile counting (128-row quarters whose cost rows are read, colquarters) / 4 (all of them without culling) */
   float c_q;             /* -log2(e) / (2 sigma2) */
   float c_s;             /* c_q * sigma2_variance */
   int32_t nonrigid_flag; /* latched once iter > nonrigid_start_iter (:289-291) */
@@ -137,10 +137,11 @@ typedef struct spb_em_params {
   float* colpart;              /* [ldx/ROW_TILE][4][nbb_pad] partial column sums */
   uint32_t* keepmask;          /* [ldx/ROW_TILE][(nbb_pad+31)/32] bit j of row rb: column j is on rb's work list, i.e. colpart[rb][.][j] is live */
   float* rowpart;              /* [seg2][8][ldx] partial row statistics */
-  float* bbox;                 /* [ldx/ROW_TILE][4][8] bounding box (lo0,lo1,lo2,hi0,hi1,hi2) of the XAHat of each 128-row quarter of each row block (valid rows only; a quarter without valid rows has lo > hi) */
+  float* bbox;                 /* [ldx/ROW_TILE][4][8] bounding box (lo0,lo1,lo2,hi0,hi1,hi2) of the XAHat of each 128-row quarter of each row block and the largest lm of the quarter (float 6) (valid rows only; a quarter without valid rows has lo > hi and lm -inf) */
   int32_t* collist;            /* [ldx/ROW_TILE][nbb_pad] per-row-block column work list */
   int32_t* colcount;           /* [ldx/ROW_TILE] list lengths */
-  uint8_t* colquarters;        /* [ldx/ROW_TILE][nbb_pad] per list position: bit q set <=> rows 128q..128q+127 of the row block can hold a non-zero weight for that column */
+  uint8_t* colquarters;        /* [ldx/ROW_TILE][nbb_pad] per list position: bit q set <=> rows 128q..128q+127 of the row block can hold a non-zero weight q = exp2(c_q d + lm) for that column (their cost rows are read) */
+  uint8_t* colspatial;         /* [ldx/ROW_TILE][nbb_pad] per list position: bit q set <=> rows 128q..128q+127 of the row block can hold a non-zero spatial weight exp2(c_s d) for that column */
   int32_t* colsplit;           /* [ldx/ROW_TILE] list positions >= colsplit[rb] hold columns whose SPATIAL weights exp(-d/(2 sigma2/variance)) are exactly 0 for the whole row block (they only need the sigma2 / full posteriors) */
   uint32_t* colmask;           /* [nbb_pad][SPB_COLMASK_WORDS] sparse mode: row blocks that can hold a non-zero weight, or NULL */
   double* UtWU;                /* [K][K] accumulator */

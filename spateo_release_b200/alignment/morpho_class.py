@@ -1159,6 +1159,7 @@ class Morpho_pairwise:
         s["bbox"] = torch.zeros((nrb, 4, 8), dtype=f32, device=dev)
         s["collist"] = torch.zeros((nrb, self._nbb_pad), dtype=torch.int32, device=dev)
         s["colquarters"] = torch.zeros((nrb, self._nbb_pad), dtype=torch.uint8, device=dev)
+        s["colspatial"] = torch.zeros((nrb, self._nbb_pad), dtype=torch.uint8, device=dev)
         s["colcount"] = torch.zeros((nrb,), dtype=torch.int32, device=dev)
         s["colsplit"] = torch.zeros((nrb,), dtype=torch.int32, device=dev)
         if self.sparse_calculation_mode:
@@ -1254,7 +1255,7 @@ class Morpho_pairwise:
         p.GT, p.UT = ptr(self._GT).value, ptr(self._UT).value
         for name in ("xa", "xb4", "Gamma", "kappa", "batch_idx", "alpha", "SigmaDiag", "lm", "mm", "VnA", "RnA", "XAHat",
                      "K_NA", "K_NA_spatial", "K_NA_sigma2", "PXB", "PXB_term", "K_NB", "colgeom", "colconst", "colpart", "keepmask",
-                     "rowpart", "bbox", "collist", "colquarters", "colcount", "colsplit", "UtWU", "UtPXB", "SigmaInv", "Sigma", "Coff", "moments", "sc",
+                     "rowpart", "bbox", "collist", "colquarters", "colspatial", "colcount", "colsplit", "UtWU", "UtPXB", "SigmaInv", "Sigma", "Coff", "moments", "sc",
                      "trace_buf"):
             t = s[name]
             setattr(p, name, None if t is None else t.data_ptr())

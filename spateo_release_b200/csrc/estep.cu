@@ -32,7 +32,7 @@ struct __align__(16) SmemLayout {
   float tile[kStages][kColStage][kRowTile];  // kColStage x 4 KB per stage
   float4 cols[kStages][kColStage][kColF4];   // per-column constants, pre-duplicated for packed math (80 B / column)
   float red[2][kConsumers / 32][32];         // sweep-1 cross-warp staging
-  uint64_t quarters[kStages];                // byte jj: live quarters of the stage's column jj (colquarters)
+  uint64_t quarters[kStages];                // byte jj of the stage's column jj: colquarters | colspatial << 4
   uint64_t full[kStages];
   uint64_t empty[kStages];
 };
@@ -61,14 +61,16 @@ __device__ __forceinline__ ColRange col_range(const int32_t* __restrict__ colcou
 }
 
 // One stage = the live quarters (512 B each) of kColStage GT rows + the columns' constants. A column's live quarters
-// (colquarters) are copied as one bulk copy per run of adjacent quarters (a 4-bit mask has at most two runs); the other
-// quarters of the slot keep stale data that the owning consumer warp never reads. Slots past the end of the slice have
-// no live quarter and take the all-zero constant entry at index NBb (the constant arrays are zero-padded). The stage's
-// masks go to sm.quarters before the arrive on the full barrier, which publishes them with the copies.
+// (colquarters: the quarters whose weights q can be non-zero) are copied as one bulk copy per run of adjacent quarters (a
+// 4-bit mask has at most two runs); the other quarters of the slot keep stale data that the owning consumer warp never
+// reads. Slots past the end of the slice have no live quarter and take the all-zero constant entry at index NBb (the
+// constant arrays are zero-padded). The stage's masks, with the spatially live quarters (colspatial) in the high nibble
+// of each byte, go to sm.quarters before the arrive on the full barrier, which publishes them with the copies.
 __device__ __forceinline__ void producer_loop(SmemLayout& sm, const float* __restrict__ GT, int64_t ldx,
                                               const int32_t* __restrict__ col_index, const int32_t* __restrict__ list,
-                                              const uint8_t* __restrict__ quarters, const float* __restrict__ colsrc,
-                                              int col_floats, int i0, ColRange cr, int NBb, int lane) {
+                                              const uint8_t* __restrict__ quarters, const uint8_t* __restrict__ spatial,
+                                              const float* __restrict__ colsrc, int col_floats, int i0, ColRange cr, int NBb,
+                                              int lane) {
   const int nst = (cr.end - cr.begin + kColStage - 1) / kColStage;
   for (int st = 0; st < nst; ++st) {
     const int s = st % kStages;
@@ -76,10 +78,11 @@ __device__ __forceinline__ void producer_loop(SmemLayout& sm, const float* __res
     const int pb = cr.begin + st * kColStage;
     const bool slot = lane < kColStage, live = slot && pb + lane < cr.end;
     const uint32_t qm = live ? quarters[pb + lane] : 0u;
+    const uint32_t wm = live ? qm | (uint32_t)spatial[pb + lane] << 4 : 0u;
     const uint32_t bytes = slot ? __popc(qm) * kQuarter * 4 + col_floats * 4 : 0u;
     const uint32_t total = __reduce_add_sync(0xffffffffu, bytes);
-    const uint32_t lo = __reduce_or_sync(0xffffffffu, lane < 4 ? qm << (8 * lane) : 0u);
-    const uint32_t hi = __reduce_or_sync(0xffffffffu, (lane >= 4 && slot) ? qm << (8 * (lane - 4)) : 0u);
+    const uint32_t lo = __reduce_or_sync(0xffffffffu, lane < 4 ? wm << (8 * lane) : 0u);
+    const uint32_t hi = __reduce_or_sync(0xffffffffu, (lane >= 4 && slot) ? wm << (8 * (lane - 4)) : 0u);
     if (lane == 0) {
       sm.quarters[s] = ((uint64_t)hi << 32) | lo;
       mbar_expect_tx(&sm.full[s], total);
@@ -102,11 +105,13 @@ __device__ __forceinline__ void producer_loop(SmemLayout& sm, const float* __res
   }
 }
 
-// A consumer warp skips a column whose quarter bit is clear (colquarters): every pair of its 128 rows with that column has
-// ex2(c_q d + lm) = +0 and ex2(c_s d) = +0 in fp32 (c_q dmin^2 < -127 for the quarter's box, lm <= 0 because alpha < 1 and
-// SigmaDiag >= 0, c_s <= c_q < 0), so sweep 1 would have reduced exact zeros and sweep 2 would have added exact zeros (an
-// accumulator that starts at +0 is never -0, so x + 0 = x). Skipping is therefore bit-identical.
-__device__ __forceinline__ bool quarter_live(uint64_t wq, int jj) { return (wq >> (8 * jj)) & 1u; }
+// A consumer warp reads the cost matrix and forms the weights q only for a column whose q bit (low nibble) is set, and forms
+// the spatial weights s only where its s bit (high nibble) is set. A clear bit means every pair of the warp's 128 rows with
+// that column has an fp32 ex2 argument below -126 (build_col_lists_kernel): ex2(c_q d + lm) = +0 or ex2(c_s d) = +0. Sweep 1
+// would have reduced exact zeros and sweep 2 would have added exact zeros (an accumulator that starts at +0 is never -0, so
+// x + 0 = x). Skipping is therefore bit-identical.
+__device__ __forceinline__ bool quarter_q(uint64_t wq, int jj) { return (wq >> (8 * jj)) & 1u; }
+__device__ __forceinline__ bool quarter_s(uint64_t wq, int jj) { return (wq >> (8 * jj + 4)) & 1u; }
 
 // ---- fp32 pairs: two moving cells per value. Hopper has no packed fp32x2 instructions, so every pair operation is two
 // scalar operations with explicit round-to-nearest (no contraction: the same bits as a packed add / mul / fma) ----------
@@ -222,7 +227,7 @@ __device__ __forceinline__ void sweep1_stage_q(const SmemLayout& sm, int s, int 
                                                u64 CQ, uint64_t wq, float (&acc)[2 * kColStage]) {
 #pragma unroll
   for (int jj = 0; jj < kColStage; ++jj) {
-    if (!quarter_live(wq, jj)) {
+    if (!quarter_q(wq, jj)) {
       acc[0 * kColStage + jj] = acc[1 * kColStage + jj] = 0.f;
       continue;
     }
@@ -242,21 +247,24 @@ __device__ __forceinline__ void sweep1_stage(const SmemLayout& sm, int s, int ti
                                              u64 CQ, u64 CS, uint64_t wq, float (&acc)[4 * kColStage]) {
 #pragma unroll
   for (int jj = 0; jj < kColStage; ++jj) {
-    if (!quarter_live(wq, jj)) {
-      acc[0 * kColStage + jj] = acc[1 * kColStage + jj] = acc[2 * kColStage + jj] = acc[3 * kColStage + jj] = 0.f;
-      continue;
-    }
+    acc[0 * kColStage + jj] = acc[1 * kColStage + jj] = acc[2 * kColStage + jj] = acc[3 * kColStage + jj] = 0.f;
+    const bool ql = quarter_q(wq, jj), sl = quarter_s(wq, jj);
+    if (!ql && !sl) continue;
     const ulonglong2 ya = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][0]);  // (y0,y0) (y1,y1)
     const ulonglong2 yb = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][1]);  // (y2,y2) (0,0)
-    const ulonglong2 g = *reinterpret_cast<const ulonglong2*>(&sm.tile[s][jj][tid * 4]);
     const u64 da = sqdist2<kDim>(R.xa0, R.xa1, R.xa2, ya.x, ya.y, yb.x);
     const u64 db = sqdist2<kDim>(R.xb0, R.xb1, R.xb2, ya.x, ya.y, yb.x);
-    const u64 sa = ex2_2(mul2(CS, da)), sb = ex2_2(mul2(CS, db));
-    const u64 qa = ex2_2(fma2(CQ, da, R.lma)), qb = ex2_2(fma2(CQ, db, R.lmb));
-    acc[0 * kColStage + jj] = hsum(add2(sa, sb));
-    acc[1 * kColStage + jj] = hsum(fma2(sa, R.mma, mul2(sb, R.mmb)));
-    acc[2 * kColStage + jj] = hsum(add2(qa, qb));
-    acc[3 * kColStage + jj] = hsum(fma2(qa, g.x, mul2(qb, g.y)));
+    if (sl) {
+      const u64 sa = ex2_2(mul2(CS, da)), sb = ex2_2(mul2(CS, db));
+      acc[0 * kColStage + jj] = hsum(add2(sa, sb));
+      acc[1 * kColStage + jj] = hsum(fma2(sa, R.mma, mul2(sb, R.mmb)));
+    }
+    if (ql) {
+      const ulonglong2 g = *reinterpret_cast<const ulonglong2*>(&sm.tile[s][jj][tid * 4]);
+      const u64 qa = ex2_2(fma2(CQ, da, R.lma)), qb = ex2_2(fma2(CQ, db, R.lmb));
+      acc[2 * kColStage + jj] = hsum(add2(qa, qb));
+      acc[3 * kColStage + jj] = hsum(fma2(qa, g.x, mul2(qb, g.y)));
+    }
   }
 }
 
@@ -298,19 +306,21 @@ __device__ __forceinline__ void sweep2_stage(const SmemLayout& sm, int s, int ti
                                              u64 CQ, u64 CS, uint64_t wq, S2Acc& A) {
 #pragma unroll
   for (int jj = 0; jj < kColStage; ++jj) {
-    if (!quarter_live(wq, jj)) continue;
+    const bool ql = quarter_q(wq, jj), sl = kSpatial && quarter_s(wq, jj);
+    if (!ql && !sl) continue;
     const ulonglong2 c0 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][0]);  // (y0,y0) (y1,y1)
     const ulonglong2 c1 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][1]);  // (y2,y2) (a,a)
-    const ulonglong2 c2 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][2]);  // (b,b)  (c,c)
-    const ulonglong2 c3 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][3]);  // (c y0, c y0) (c y1, c y1)
-    const ulonglong2 g = *reinterpret_cast<const ulonglong2*>(&sm.tile[s][jj][tid * 4]);
     const u64 da = sqdist2<kDim>(R.xa0, R.xa1, R.xa2, c0.x, c0.y, c1.x);
     const u64 db = sqdist2<kDim>(R.xb0, R.xb1, R.xb2, c0.x, c0.y, c1.x);
-    if constexpr (kSpatial) {
+    if (sl) {
       const u64 sa = ex2_2(mul2(CS, da)), sb = ex2_2(mul2(CS, db));
       A.spa = fma2(sa, c1.y, A.spa);
       A.spb = fma2(sb, c1.y, A.spb);
     }
+    if (!ql) continue;
+    const ulonglong2 c2 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][2]);  // (b,b)  (c,c)
+    const ulonglong2 c3 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][3]);  // (c y0, c y0) (c y1, c y1)
+    const ulonglong2 g = *reinterpret_cast<const ulonglong2*>(&sm.tile[s][jj][tid * 4]);
     const u64 qa = ex2_2(fma2(CQ, da, R.lma)), qb = ex2_2(fma2(CQ, db, R.lmb));
     const u64 ta = mul2(qa, c2.x), tb = mul2(qb, c2.x);
     A.s2a = add2(A.s2a, ta);
@@ -352,7 +362,8 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
                     const float* __restrict__ colgeom, const float* __restrict__ XA, const float* __restrict__ lm,
                     const float* __restrict__ mm, const spb_scalars* __restrict__ sc, float* __restrict__ colpart,
                     int NBb, int nbb_pad, const int32_t* __restrict__ collist, const uint8_t* __restrict__ colquarters,
-                    const int32_t* __restrict__ colcount, const int32_t* __restrict__ colsplit) {
+                    const uint8_t* __restrict__ colspatial, const int32_t* __restrict__ colcount,
+                    const int32_t* __restrict__ colsplit) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   SmemLayout& sm = *reinterpret_cast<SmemLayout*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -361,6 +372,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   const ColRange cr = col_range(colcount, rb, seg, gridDim.y);
   const int32_t* list = collist + (int64_t)rb * nbb_pad;
   const uint8_t* quarters = colquarters + (int64_t)rb * nbb_pad;
+  const uint8_t* spatial = colspatial + (int64_t)rb * nbb_pad;
   const int32_t* col_index = batch_cols(batch_base, sc, NBb);
   const int split = colsplit[rb];  // list positions >= split: spatially dead columns
   if (cr.begin >= cr.end) return;
@@ -374,7 +386,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   __syncthreads();
 
   if (warp == kConsumers / 32) {
-    producer_loop(sm, GT, ldx, col_index, list, quarters, colgeom, 8, i0, cr, NBb, lane);
+    producer_loop(sm, GT, ldx, col_index, list, quarters, spatial, colgeom, 8, i0, cr, NBb, lane);
     return;
   }
   // ---- consumers: 4 rows per thread = 2 packed row pairs ----
@@ -387,7 +399,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
     const int pb = cr.begin + st * kColStage;
     constexpr int NV = 4 * kColStage;  // partial sums per thread per stage, index v * kColStage + jj
     const int buf = st & 1;
-    const uint64_t wq = sm.quarters[s] >> warp;  // bit 8 jj: this warp's quarter of column jj is live
+    const uint64_t wq = sm.quarters[s] >> warp;  // bits 8 jj, 8 jj + 4: this warp's q and s bits of column jj
     if (pb >= split) {
       // all columns of the stage are spatially dead: sums 0 and 1 are exact zeros, only 2 and 3 are computed and reduced
       constexpr int NQ = 2 * kColStage;
@@ -507,7 +519,8 @@ estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
                     const float* __restrict__ colconst, const float* __restrict__ XA, const float* __restrict__ lm,
                     const spb_scalars* __restrict__ sc, float* __restrict__ rowpart, int NBb, int nbb_pad,
                     const int32_t* __restrict__ collist, const uint8_t* __restrict__ colquarters,
-                    const int32_t* __restrict__ colcount, const int32_t* __restrict__ colsplit) {
+                    const uint8_t* __restrict__ colspatial, const int32_t* __restrict__ colcount,
+                    const int32_t* __restrict__ colsplit) {
   extern __shared__ __align__(128) uint8_t smem_raw[];
   SmemLayout& sm = *reinterpret_cast<SmemLayout*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -517,6 +530,7 @@ estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   const ColRange cr = col_range(colcount, rb, seg, gridDim.y);
   const int32_t* list = collist + (int64_t)rb * nbb_pad;
   const uint8_t* quarters = colquarters + (int64_t)rb * nbb_pad;
+  const uint8_t* spatial = colspatial + (int64_t)rb * nbb_pad;
   const int32_t* col_index = batch_cols(batch_base, sc, NBb);
   const int j_begin = cr.begin, j_end = cr.end;
   if (tid == 0) {
@@ -529,7 +543,8 @@ estep_sweep2_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   __syncthreads();
   const int nst = j_begin < j_end ? (j_end - j_begin + kColStage - 1) / kColStage : 0;
   if (warp == kConsumers / 32) {
-    if (j_begin < j_end) producer_loop(sm, GT, ldx, col_index, list, quarters, colconst, SPB_COLCONST_FLOATS, i0, cr, NBb, lane);
+    if (j_begin < j_end)
+      producer_loop(sm, GT, ldx, col_index, list, quarters, spatial, colconst, SPB_COLCONST_FLOATS, i0, cr, NBb, lane);
     return;
   }
   const u64 CQ = pk(sc->c_q, sc->c_q), CS = pk(sc->c_s, sc->c_s);
@@ -651,12 +666,12 @@ row_stats_p2p_kernel(const uint64_t* __restrict__ peer_stat, int parity, int ran
   grid_reduce_ordered<4>(v, red_scratch, red_counter, sc->sums, false);
 }
 
-// bounding box of the current positions of each 128-row quarter of each row block (valid rows only): warp w reduces the
-// rows of consumer warp w of the sweeps
-__global__ void __launch_bounds__(kConsumers) block_bounds_kernel(const float* __restrict__ XA, int ldx, int NA,
-                                                                  float* __restrict__ bbox) {
+// bounding box of the current positions of each 128-row quarter of each row block and the largest row term lm of the
+// quarter (valid rows only): warp w reduces the rows of consumer warp w of the sweeps
+__global__ void __launch_bounds__(kConsumers) block_bounds_kernel(const float* __restrict__ XA, const float* __restrict__ lm,
+                                                                  int ldx, int NA, float* __restrict__ bbox) {
   const int rb = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f};
+  float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f}, lmax = -INFINITY;
   for (int q = 0; q < 4; ++q) {
     const int i = rb * kRowTile + threadIdx.x * 4 + q;
     if (i < NA) {
@@ -666,8 +681,12 @@ __global__ void __launch_bounds__(kConsumers) block_bounds_kernel(const float* _
         lo[d] = fminf(lo[d], x);
         hi[d] = fmaxf(hi[d], x);
       }
+      lmax = fmaxf(lmax, lm[i]);
     }
   }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) lmax = fmaxf(lmax, __shfl_xor_sync(0xffffffffu, lmax, o));
+  if (lane == 0) bbox[(rb * 4 + warp) * 8 + 6] = lmax;
 #pragma unroll
   for (int d = 0; d < 3; ++d) {
 #pragma unroll
@@ -693,12 +712,15 @@ __device__ __forceinline__ float box_dist2(const float (&lo)[3], const float (&h
 }
 
 // Per row block: order-preserving compaction of the columns that are not provably zero for every row of the block.
-// A column j is dropped when c_q * dmin^2 < -127 (log2 domain, with a 1e-5 relative safety margin), dmin = distance from
-// y_j to the block's bounding box: then ex2(c_q d + lm) and ex2(c_s d) flush to +0 for every pair of the block (lm <= 0,
-// c_s <= c_q < 0), so the dropped pairs would have added exact zeros. The same test against the box of each 128-row quarter
-// gives the listed column's quarter mask (colquarters): the sweeps read and compute only the live quarters of a column.
-// The list itself is built from the block's box, so the list, its live / dead split and the column segments of the sweeps
-// do not depend on the quarter masks, and neither does the order in which any sum is formed.
+// With dmin the distance from y_j to a bounding box and lmax the largest row term lm = log2(alpha e^(-SigmaDiag/sigma2))
+// of its rows, every pair (i, j) of the box's rows has an fp32 ex2 argument below -126 in the sweeps
+//   for the weight q = ex2(c_q d + lm)   when  c_q dmin^2 + lmax < -127,
+//   for the spatial weight s = ex2(c_s d) when  c_s dmin^2 < -127
+// (log2 domain; the 1e-5 relative margin on c_q and c_s and the one unit between -127 and -126 cover the rounding of d and
+// of the fma), so that weight flushes to +0. The cost matrix enters only through q g, so it is read only where q can be
+// non-zero. Per 128-row quarter the two tests give the listed column's quarter masks: colquarters (q: the quarter's cost
+// rows are read) and colspatial (s is formed). A column is listed when either test passes against the block's box; it is
+// spatially live (before colsplit) when the s test passes. Dropped pairs would have added exact zeros.
 // One CTA per row block, 32 warps, each warp owns a contiguous range of columns: pass 1 evaluates the block test once (the
 // keep bits go to shared memory), one block barrier turns the per-warp counts into offsets, pass 2 scatters the listed
 // columns with their quarter masks. The keep bits are also published (keepmask): col_finalize folds only the partial column
@@ -723,7 +745,7 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
                                                                        int gstride, int gstep,
                                                                        int NBb, spb_scalars* __restrict__ sc, int cull,
                                                                        int32_t* __restrict__ collist, uint8_t* __restrict__ colquarters,
-                                                                       int32_t* __restrict__ colcount, int32_t* __restrict__ colsplit,
+                                                                       uint8_t* __restrict__ colspatial, int32_t* __restrict__ colcount, int32_t* __restrict__ colsplit,
                                                                        int nbb_pad, uint32_t* __restrict__ colmask,
                                                                        uint32_t* __restrict__ keepmask, int kstride) {
   extern __shared__ uint32_t keep_bits[];  // [2][nwords]: one word per 32 columns — kept at all | spatially live
@@ -731,10 +753,13 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
   __shared__ int live_quarters;
   const int rb = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const float cq = sc->c_q * (1.0f - 1e-5f);
-  const float cs = sc->c_s * (1.0f - 1e-5f);  // c_s = c_q * sigma2_variance <= c_q: the spatial weight dies first
+  const float cs = sc->c_s * (1.0f - 1e-5f);  // c_s = c_q * sigma2_variance
   float qlo[4][3], qhi[4][3], lo[3], hi[3];   // quarter boxes and the block's box (their union)
+  float qlm[4], blm = -INFINITY;              // largest row term of each quarter and of the block
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
+    qlm[q] = bbox[(rb * 4 + q) * 8 + 6];
+    blm = fmaxf(blm, qlm[q]);
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
       qlo[q][d] = bbox[(rb * 4 + q) * 8 + d];
@@ -767,8 +792,8 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
         keep = live = true;
         if (cull) {
           const float d2 = box_dist2(lo, hi, yy[u]);
-          keep = cq * d2 >= -127.0f;
-          live = cs * d2 >= -127.0f;  // implies keep
+          live = cs * d2 >= -127.0f;
+          keep = live || cq * d2 + blm >= -127.0f;
         }
       }
       const uint32_t bits = __ballot_sync(0xffffffffu, keep), lbits = __ballot_sync(0xffffffffu, live);
@@ -803,7 +828,8 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
   off_dead += total_live;  // the spatially dead columns follow the live ones in the list
   int32_t* list = collist + (int64_t)rb * nbb_pad;
   uint8_t* qlist = colquarters + (int64_t)rb * nbb_pad;
-  int nq = 0;  // live quarters of this lane's listed columns
+  uint8_t* slist = colspatial + (int64_t)rb * nbb_pad;
+  int nq = 0;  // quarters of this lane's listed columns whose cost rows are read
   float ynext[3];
   if (w0 < w1) load_col(geom, gstride, gstep, w0 * 32 + lane, w0 * 32 + lane < NBb, cull, ynext);
   for (int wd = w0; wd < w1; ++wd) {
@@ -816,14 +842,19 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
     if ((lbits >> lane) & 1u) pos = off_live + __popc(lbits & below);
     else if ((dbits >> lane) & 1u) pos = off_dead + __popc(dbits & below);
     if (pos >= 0) {
-      uint32_t qm = 0xFu;  // without culling every quarter of every column is read
+      uint32_t qm = 0xFu, sm = 0xFu;  // without culling every quarter of every column is read and computed
       if (cull) {
-        qm = 0u;
+        qm = sm = 0u;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) qm |= (cq * box_dist2(qlo[q], qhi[q], y) >= -127.0f) ? 1u << q : 0u;
+        for (int q = 0; q < 4; ++q) {
+          const float d2 = box_dist2(qlo[q], qhi[q], y);
+          qm |= (cq * d2 + qlm[q] >= -127.0f) ? 1u << q : 0u;
+          sm |= (cs * d2 >= -127.0f) ? 1u << q : 0u;
+        }
       }
       list[pos] = j;
       qlist[pos] = (uint8_t)qm;
+      slist[pos] = (uint8_t)sm;
       nq += __popc(qm);
     }
     if (lane == 0) keepmask[(int64_t)rb * kstride + wd] = bits;  // col_finalize folds only the listed (row block, column) partials
@@ -1237,7 +1268,7 @@ int launch_sweep1(const spb_em_params* p, const int32_t* bidx, cudaStream_t st) 
   }
   dim3 grid(p->ldx / kRowTile, p->seg1);
   estep_sweep1_kernel<DIM><<<grid, kThreads, sizeof(SmemLayout), st>>>(p->GT, p->ldx, bidx, p->colgeom, p->XAHat, p->lm, p->mm, p->sc,
-                                                                      p->colpart, p->NBb, p->nbb_pad, p->collist, p->colquarters, p->colcount,
+                                                                      p->colpart, p->NBb, p->nbb_pad, p->collist, p->colquarters, p->colspatial, p->colcount,
                                                                       p->colsplit);
   return 0;
 }
@@ -1255,7 +1286,7 @@ int launch_sweep2(const spb_em_params* p, const int32_t* bidx, cudaStream_t st) 
   }
   dim3 grid(p->ldx / kRowTile, p->seg2);
   estep_sweep2_kernel<SP, DIM><<<grid, kThreads, sizeof(SmemLayout), st>>>(p->GT, p->ldx, bidx, p->colconst, p->XAHat, p->lm, p->sc,
-                                                                          p->rowpart, p->NBb, p->nbb_pad, p->collist, p->colquarters, p->colcount,
+                                                                          p->rowpart, p->NBb, p->nbb_pad, p->collist, p->colquarters, p->colspatial, p->colcount,
                                                                           p->colsplit);
   return 0;
 }
@@ -1279,7 +1310,7 @@ extern "C" int spb_gather_cols(const spb_em_params* p, int32_t iter, void* strea
 
 extern "C" int spb_estep_col_lists(const spb_em_params* p, void* stream) {
   const int nrb = p->ldx / kRowTile;
-  block_bounds_kernel<<<nrb, kConsumers, 0, (cudaStream_t)stream>>>(p->XAHat, p->ldx, p->NA, p->bbox);
+  block_bounds_kernel<<<nrb, kConsumers, 0, (cudaStream_t)stream>>>(p->XAHat, p->lm, p->ldx, p->NA, p->bbox);
   SPB_CHECK_LAUNCH();
   // sparse mode also records, per column, which row blocks can hold a non-zero weight (col_select skips the others)
   uint32_t* colmask = (p->sparse_k > 0 && nrb <= 32 * SPB_COLMASK_WORDS) ? p->colmask : nullptr;
@@ -1299,7 +1330,7 @@ extern "C" int spb_estep_col_lists(const spb_em_params* p, void* stream) {
   const bool all_cols = !(p->svi && p->batch_idx);  // the iteration's columns are the fixed cells themselves, in order
   build_col_lists_kernel<<<nrb, kListThreads, smem, (cudaStream_t)stream>>>(
       p->bbox, all_cols ? p->xb4 : p->colgeom, all_cols ? 4 : 8, all_cols ? 1 : 2, p->NBb, p->sc, p->cull, p->collist,
-      p->colquarters, p->colcount, p->colsplit, p->nbb_pad, colmask, p->keepmask, (p->nbb_pad + 31) / 32);
+      p->colquarters, p->colspatial, p->colcount, p->colsplit, p->nbb_pad, colmask, p->keepmask, (p->nbb_pad + 31) / 32);
   SPB_CHECK_LAUNCH();
   return 0;
 }
