@@ -134,8 +134,10 @@ typedef struct spb_em_params {
   float* K_NB;                 /* [NBb] */
   float* colgeom;              /* [nbb_pad][8] (y0,y0,y1,y1,y2,y2,0,0): this iteration's columns, duplicated for f32x2 */
   float* colconst;             /* [nbb_pad][SPB_COLCONST_FLOATS] (y0,y0,y1,y1, y2,y2,a,a, b,b,c,c, cy0,cy0,cy1,cy1, cy2,cy2,tau,tau); zero beyond NBb */
-  float* colpart;              /* [ldx/ROW_TILE][4][nbb_pad] partial column sums */
-  uint32_t* keepmask;          /* [ldx/ROW_TILE][(nbb_pad+31)/32] bit j of row rb: column j is on rb's work list, i.e. colpart[rb][.][j] is live */
+  float* colpart;              /* [ldx/ROW_TILE][4][nbb_pad] partial column sums of each row block, by position in its work list (sums 0 and 1 of the spatially dead columns are not stored: they are zero) */
+  uint32_t* keepmask;          /* [ldx/ROW_TILE][(nbb_pad+31)/32] bit j of row rb: column j is on rb's work list, i.e. rb has column sums of j */
+  uint32_t* livemask;          /* [ldx/ROW_TILE][(nbb_pad+31)/32] bit j of row rb: column j is on rb's work list before colsplit (spatially live) */
+  int32_t* keepoff;            /* [ldx/ROW_TILE][(nbb_pad+31)/32][2] list position of the first spatially live / dead listed column of each 32-column word */
   float* rowpart;              /* [seg2][8][ldx] partial row statistics */
   float* bbox;                 /* [ldx/ROW_TILE][4][8] bounding box (lo0,lo1,lo2,hi0,hi1,hi2) of the XAHat of each 128-row quarter of each row block and the largest lm of the quarter (float 6) (valid rows only; a quarter without valid rows has lo > hi and lm -inf) */
   int32_t* collist;            /* [ldx/ROW_TILE][nbb_pad] per-row-block column work list */

@@ -108,7 +108,8 @@ def pair_device_bytes(n_moving: int, n_fixed: int, n_genes: int, chunk_cols: Opt
     pad = -(-chunk_cols // 8) * 8 + 8
     per_col = (
         4 * ldx                                  # cost chunk
-        + nrb * (4 * 4 + 4 + 2) + nrb // 8 + 1   # colpart [nrb][4], collist, colquarters, colspatial, keepmask bits
+        + nrb * (4 * 4 + 4 + 2) + nrb // 2 + 1   # colpart [nrb][4], collist, colquarters, colspatial; per 32 columns:
+                                                 # keepmask and livemask bits, the two list offsets (keepoff)
         + 4 + 8 * 4 + _capi.CONST["SPB_COLCONST_FLOATS"] * 4 + _capi.CONST["SPB_COLMASK_WORDS"] * 4  # K_NB, colgeom, colconst, colmask
         + 2 * 4 * gp + 2 * 4                     # gathered tf32 hi / lo operands, row term, label
     )

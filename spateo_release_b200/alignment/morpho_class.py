@@ -1151,6 +1151,8 @@ class Morpho_pairwise:
         s["colconst"] = torch.zeros((self._nbb_pad, _capi.CONST["SPB_COLCONST_FLOATS"]), dtype=f32, device=dev)
         s["colpart"] = torch.zeros((nrb, 4, self._nbb_pad), dtype=f32, device=dev)
         s["keepmask"] = torch.zeros((nrb, (self._nbb_pad + 31) // 32), dtype=torch.int32, device=dev)
+        s["livemask"] = torch.zeros_like(s["keepmask"])
+        s["keepoff"] = torch.zeros((nrb, (self._nbb_pad + 31) // 32, 2), dtype=torch.int32, device=dev)
         n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
         seg1 = self._choose_segments(nrb, min(nbb, width), n_sms)
         seg2 = self._choose_segments(nrb, min(nbb, width), n_sms)
@@ -1255,7 +1257,7 @@ class Morpho_pairwise:
         p.GT, p.UT = ptr(self._GT).value, ptr(self._UT).value
         for name in ("xa", "xb4", "Gamma", "kappa", "batch_idx", "alpha", "SigmaDiag", "lm", "mm", "VnA", "RnA", "XAHat",
                      "K_NA", "K_NA_spatial", "K_NA_sigma2", "PXB", "PXB_term", "K_NB", "colgeom", "colconst", "colpart", "keepmask",
-                     "rowpart", "bbox", "collist", "colquarters", "colspatial", "colcount", "colsplit", "UtWU", "UtPXB", "SigmaInv", "Sigma", "Coff", "moments", "sc",
+                     "livemask", "keepoff", "rowpart", "bbox", "collist", "colquarters", "colspatial", "colcount", "colsplit", "UtWU", "UtPXB", "SigmaInv", "Sigma", "Coff", "moments", "sc",
                      "trace_buf"):
             t = s[name]
             setattr(p, name, None if t is None else t.data_ptr())

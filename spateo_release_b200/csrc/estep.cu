@@ -375,6 +375,9 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
   const uint8_t* spatial = colspatial + (int64_t)rb * nbb_pad;
   const int32_t* col_index = batch_cols(batch_base, sc, NBb);
   const int split = colsplit[rb];  // list positions >= split: spatially dead columns
+  // partials are stored by list position: a stage's kColStage values of one sum are one aligned 32-byte sector
+  // (segments begin at multiples of kColStage, nbb_pad is a multiple of 8)
+  float* part = colpart + (int64_t)rb * 4 * nbb_pad;
   if (cr.begin >= cr.end) return;
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
@@ -401,7 +404,8 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
     const int buf = st & 1;
     const uint64_t wq = sm.quarters[s] >> warp;  // bits 8 jj, 8 jj + 4: this warp's q and s bits of column jj
     if (pb >= split) {
-      // all columns of the stage are spatially dead: sums 0 and 1 are exact zeros, only 2 and 3 are computed and reduced
+      // all columns of the stage are spatially dead: sums 0 and 1 are exact zeros (not stored: col_finalize knows them from
+      // the list position), only 2 and 3 are computed and reduced
       constexpr int NQ = 2 * kColStage;
       float acc[NQ];
       sweep1_stage_q<kDim>(sm, s, tid, R, CQ, wq, acc);
@@ -411,17 +415,12 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
       constexpr int kShiftQ = (NQ == 32) ? 0 : (NQ == 16 ? 1 : 2);
       if ((lane & ((1 << kShiftQ) - 1)) == 0) sm.red[buf][warp][lane >> kShiftQ] = acc[0];
       named_bar_sync(1, kConsumers);
-      if (warp == 0) {
-        if (lane < NQ) {
-          float t = 0.f;
+      if (warp == 0 && lane < NQ) {
+        float t = 0.f;
 #pragma unroll
-          for (int w = 0; w < kConsumers / 32; ++w) t += sm.red[buf][w][lane];
-          const int v = 2 + lane / kColStage, jj = lane % kColStage;
-          if (pb + jj < cr.end) colpart[((int64_t)rb * 4 + v) * nbb_pad + list[pb + jj]] = t;
-        } else if (lane < 2 * NQ) {
-          const int v = (lane - NQ) / kColStage, jj = (lane - NQ) % kColStage;
-          if (pb + jj < cr.end) colpart[((int64_t)rb * 4 + v) * nbb_pad + list[pb + jj]] = 0.f;
-        }
+        for (int w = 0; w < kConsumers / 32; ++w) t += sm.red[buf][w][lane];
+        const int v = 2 + lane / kColStage, jj = lane % kColStage;
+        if (pb + jj < cr.end) part[(int64_t)v * nbb_pad + pb + jj] = t;
       }
       continue;
     }
@@ -438,7 +437,7 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
 #pragma unroll
       for (int w = 0; w < kConsumers / 32; ++w) t += sm.red[buf][w][lane];
       const int v = lane / kColStage, jj = lane % kColStage;
-      if (pb + jj < cr.end) colpart[((int64_t)rb * 4 + v) * nbb_pad + list[pb + jj]] = t;
+      if (pb + jj < cr.end) part[(int64_t)v * nbb_pad + pb + jj] = t;
     }
   }
 }
@@ -450,30 +449,44 @@ estep_sweep1_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __
 // row-block partials per column is a chain of dependent loads otherwise) and combine through shared memory in fp64.
 constexpr int kFinWarps = 8;
 __global__ void __launch_bounds__(32 * kFinWarps)
-col_finalize_kernel(const float* __restrict__ colpart, const uint32_t* __restrict__ keepmask, int kstride, int nrb, int nbb_pad,
+col_finalize_kernel(const float* __restrict__ colpart, const uint32_t* __restrict__ keepmask,
+                    const uint32_t* __restrict__ livemask, const int2* __restrict__ keepoff, int kstride, int nrb, int nbb_pad,
                     int NBb, const float* __restrict__ colgeom,
                     const spb_scalars* __restrict__ sc, float* __restrict__ colconst, float* __restrict__ K_NB) {
   __shared__ double part[kFinWarps][4][32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int j = blockIdx.x * 32 + lane;
+  const uint32_t below = (1u << lane) - 1u;
   double C[4] = {0, 0, 0, 0};
   // a (row block, column) partial exists only if the column is on the row block's list; the others are never written or read
-  // (this warp's row blocks: warp, warp + kFinWarps, ...; lane t fetches the mask word of the t-th one, the words are then
-  // broadcast, and four row blocks' loads are in flight before the first add: the fold stays in row-block order)
+  // (this warp's row blocks: warp, warp + kFinWarps, ...; lane t fetches the mask words and list offsets of the t-th one, they
+  // are then broadcast, and four row blocks' loads are in flight before the first add: the fold stays in row-block order).
+  // Sweep 1 stored the partials by list position: the column's position is the offset of its group (spatially live / dead)
+  // in this 32-column word plus the listed columns of the group below it (build_col_lists_kernel's compaction). A spatially
+  // dead column's sums 0 and 1 are exact zeros and were not stored.
   const int nmine = (nrb - warp + kFinWarps - 1) / kFinWarps;
   for (int base = 0; base < nmine; base += 32) {
     const int t = base + lane;
-    const uint32_t mymask = t < nmine ? keepmask[(int64_t)(warp + t * kFinWarps) * kstride + blockIdx.x] : 0u;
+    const int64_t w = (int64_t)(warp + t * kFinWarps) * kstride + blockIdx.x;
+    const uint32_t mymask = t < nmine ? keepmask[w] : 0u;
+    const uint32_t mylive = t < nmine ? livemask[w] : 0u;
+    const int2 myoff = t < nmine ? keepoff[w] : make_int2(0, 0);
     const int cnt = min(32, nmine - base);
     for (int u0 = 0; u0 < cnt; u0 += 4) {
       float tmp[4][4];
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
-        const uint32_t bits = __shfl_sync(0xffffffffu, mymask, (u0 + u) & 31);
+        const int src = (u0 + u) & 31;
+        const uint32_t bits = __shfl_sync(0xffffffffu, mymask, src);
+        const uint32_t lbits = __shfl_sync(0xffffffffu, mylive, src);
+        const int off_live = __shfl_sync(0xffffffffu, myoff.x, src), off_dead = __shfl_sync(0xffffffffu, myoff.y, src);
         const bool on = (u0 + u < cnt) && ((bits >> lane) & 1u);
+        const bool live = (lbits >> lane) & 1u;
+        const int pos = live ? off_live + __popc(lbits & below) : off_dead + __popc(bits & ~lbits & below);
         const int rb = warp + (base + u0 + u) * kFinWarps;
+        const float* p = colpart + (int64_t)rb * 4 * nbb_pad + pos;
 #pragma unroll
-        for (int v = 0; v < 4; ++v) tmp[u][v] = on ? colpart[((int64_t)rb * 4 + v) * nbb_pad + j] : 0.f;
+        for (int v = 0; v < 4; ++v) tmp[u][v] = (on && (live || v >= 2)) ? p[(int64_t)v * nbb_pad] : 0.f;
       }
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
@@ -723,9 +736,10 @@ __device__ __forceinline__ float box_dist2(const float (&lo)[3], const float (&h
 // spatially live (before colsplit) when the s test passes. Dropped pairs would have added exact zeros.
 // One CTA per row block, 32 warps, each warp owns a contiguous range of columns: pass 1 evaluates the block test once (the
 // keep bits go to shared memory), one block barrier turns the per-warp counts into offsets, pass 2 scatters the listed
-// columns with their quarter masks. The keep bits are also published (keepmask): col_finalize folds only the partial column
-// sums that sweep 1 wrote, so the dropped (row block, column) combinations are neither zeroed (a 157-313 MB write per
-// iteration) nor read.
+// columns with their quarter masks. The keep bits, the spatially live bits and each word's two list offsets are also
+// published (keepmask, livemask, keepoff): col_finalize folds only the partial column sums that sweep 1 wrote, so the dropped
+// (row block, column) combinations are neither zeroed (a 157-313 MB write per iteration) nor read, and finds each partial
+// at its list position (sweep 1 stores them there, one full 32-byte sector per stage and sum instead of 4-byte scatters).
 constexpr int kListThreads = 1024;
 // geom: one record per column, `gstride` floats apart, coordinate d at float offset d * gstep (the 16-byte xb4 records when the
 // columns are all fixed cells: half the L2 traffic of the duplicated colgeom layout, which every row block re-reads in full)
@@ -747,7 +761,8 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
                                                                        int32_t* __restrict__ collist, uint8_t* __restrict__ colquarters,
                                                                        uint8_t* __restrict__ colspatial, int32_t* __restrict__ colcount, int32_t* __restrict__ colsplit,
                                                                        int nbb_pad, uint32_t* __restrict__ colmask,
-                                                                       uint32_t* __restrict__ keepmask, int kstride) {
+                                                                       uint32_t* __restrict__ keepmask, uint32_t* __restrict__ livemask,
+                                                                       int2* __restrict__ keepoff, int kstride) {
   extern __shared__ uint32_t keep_bits[];  // [2][nwords]: one word per 32 columns — kept at all | spatially live
   __shared__ int warp_cnt[2][32];
   __shared__ int live_quarters;
@@ -857,7 +872,11 @@ __global__ void __launch_bounds__(kListThreads) build_col_lists_kernel(const flo
       slist[pos] = (uint8_t)sm;
       nq += __popc(qm);
     }
-    if (lane == 0) keepmask[(int64_t)rb * kstride + wd] = bits;  // col_finalize folds only the listed (row block, column) partials
+    if (lane == 0) {  // col_finalize folds only the listed (row block, column) partials and finds them by list position
+      keepmask[(int64_t)rb * kstride + wd] = bits;
+      livemask[(int64_t)rb * kstride + wd] = lbits;
+      keepoff[(int64_t)rb * kstride + wd] = make_int2(off_live, off_dead);
+    }
     if (((bits >> lane) & 1u) && colmask != nullptr && rb < 32 * SPB_COLMASK_WORDS)
       atomicOr(colmask + (int64_t)j * SPB_COLMASK_WORDS + (rb >> 5), 1u << (rb & 31));
     off_live += __popc(lbits);
@@ -1330,14 +1349,16 @@ extern "C" int spb_estep_col_lists(const spb_em_params* p, void* stream) {
   const bool all_cols = !(p->svi && p->batch_idx);  // the iteration's columns are the fixed cells themselves, in order
   build_col_lists_kernel<<<nrb, kListThreads, smem, (cudaStream_t)stream>>>(
       p->bbox, all_cols ? p->xb4 : p->colgeom, all_cols ? 4 : 8, all_cols ? 1 : 2, p->NBb, p->sc, p->cull, p->collist,
-      p->colquarters, p->colspatial, p->colcount, p->colsplit, p->nbb_pad, colmask, p->keepmask, (p->nbb_pad + 31) / 32);
+      p->colquarters, p->colspatial, p->colcount, p->colsplit, p->nbb_pad, colmask, p->keepmask, p->livemask,
+      reinterpret_cast<int2*>(p->keepoff), (p->nbb_pad + 31) / 32);
   SPB_CHECK_LAUNCH();
   return 0;
 }
 
 extern "C" int spb_estep_sweep1(const spb_em_params* p, int32_t iter, void* stream) {
   int rc;
-  // writes the partial column sums of every (row block, listed column) combination; col_finalize reads exactly those (keepmask)
+  // writes the partial column sums of every (row block, listed column) combination by list position; col_finalize reads
+  // exactly those (keepmask, livemask, keepoff)
   if (p->D == 2) rc = launch_sweep1<2>(p, gt_batch_ptr(p, iter), (cudaStream_t)stream);
   else rc = launch_sweep1<>(p, gt_batch_ptr(p, iter), (cudaStream_t)stream);
   if (rc) return rc;
@@ -1347,7 +1368,7 @@ extern "C" int spb_estep_sweep1(const spb_em_params* p, int32_t iter, void* stre
 
 extern "C" int spb_col_finalize(const spb_em_params* p, void* stream) {
   col_finalize_kernel<<<(p->NBb + 31) / 32, 32 * kFinWarps, 0, (cudaStream_t)stream>>>(
-      p->colpart, p->keepmask, (p->nbb_pad + 31) / 32, p->ldx / kRowTile, p->nbb_pad, p->NBb, p->colgeom, p->sc, p->colconst, p->K_NB);
+      p->colpart, p->keepmask, p->livemask, reinterpret_cast<const int2*>(p->keepoff), (p->nbb_pad + 31) / 32, p->ldx / kRowTile, p->nbb_pad, p->NBb, p->colgeom, p->sc, p->colconst, p->K_NB);
   SPB_CHECK_LAUNCH();
   return 0;
 }
