@@ -17,6 +17,7 @@ if [ "$TOOL" = memcheck ] || [ "$TOOL" = all ]; then
   run memcheck tests/test_gpu_parity.py -k "$WIDE"
   run memcheck tests/test_gpu_gram.py -k "64-7000 or 257-4100 or 15-5000 or 3-900"
   run memcheck tests/test_gpu_shard.py -k "1]"
+  run memcheck tests/test_gpu_shard_options.py -k "mapping_from_identical_state or svi_estep_from_identical_state"
 fi
 if [ "$TOOL" = racecheck ] || [ "$TOOL" = all ]; then
   run racecheck tests/test_gpu_parity.py -k "$NARROW"

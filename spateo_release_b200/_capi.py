@@ -133,6 +133,7 @@ def load_library():
         "spb_estep_col_select": ([EP, I32, P], C.c_int),
         "spb_sparse_P_emit": ([EP, I32, P, P, P], C.c_int),
         "spb_posterior_argmax": ([EP, I32, P, P, P], C.c_int),
+        "spb_posterior_argmax_mapped": ([EP, I32, P, P, P, P], C.c_int),
         "spb_materialize_P": ([EP, I32, P, I64, P], C.c_int),
         "spb_iter_begin": ([EP, I32, P], C.c_int),
         "spb_update_gamma_alpha": ([EP, P], C.c_int),

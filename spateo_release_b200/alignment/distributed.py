@@ -221,6 +221,33 @@ def column_block(n_cols: int, rank: int, world: int):
     return (n_cols * rank) // world, (n_cols * (rank + 1)) // world
 
 
+def assemble_columns(parts: List[np.ndarray], positions: List[np.ndarray], n_out: int, fill=0) -> np.ndarray:
+    """Per-column rows of a column-sharded E-step in the unsharded column order: row ``k`` of rank r's ``parts[r]`` goes to
+    output column ``positions[r][k]``; positions of -1 (null columns) and rows beyond ``len(positions[r])`` (padding of
+    the gather) are dropped. Returns [n_out, ...]; columns no rank holds keep ``fill``."""
+    out = np.full((n_out,) + parts[0].shape[1:], fill, dtype=parts[0].dtype)
+    for part, pos in zip(parts, positions):
+        pos = np.asarray(pos)
+        keep = pos >= 0
+        out[pos[keep]] = part[: pos.shape[0]][keep]
+    return out
+
+
+def all_gather_rows(t: torch.Tensor) -> List[torch.Tensor]:
+    """Every rank's ``t`` ([n_r, ...], n_r may differ between ranks), in rank order: one ``all_gather`` of slabs padded to
+    the largest n_r (the caller knows which rows are real; ``assemble_columns`` drops the padding)."""
+    world = dist.get_world_size()
+    n = torch.tensor([t.shape[0]], dtype=torch.int64, device=t.device)
+    sizes = [torch.zeros_like(n) for _ in range(world)]
+    dist.all_gather(sizes, n)
+    width = int(max(int(q.item()) for q in sizes))
+    slab = torch.zeros((width,) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
+    slab[: t.shape[0]] = t
+    parts = [torch.zeros_like(slab) for _ in range(world)]
+    dist.all_gather(parts, slab)
+    return [q[: int(m.item())] for q, m in zip(parts, sizes)]
+
+
 _HOST_INIT_FIELDS = ("coordsA", "init_R", "init_t", "inlier_A", "inlier_B", "inlier_P", "sigma2", "_sigma2_init",
                      "probability_parameters", "samples_s", "outlier_s", "sigma2_variance_decress", "batch_perm")
 
@@ -235,16 +262,31 @@ def morpho_align_pair_sharded(fixed, moving, mode: str = "auto", device=None, **
     INSIDE the row-finalize kernel by reading the peers' partial vectors over NVLink in rank order (bit-identical replicas, no
     separate collective); ``mode="nccl"``: ``all_reduce`` + a finishing kernel (the baseline). The M-step runs replicated.
 
-    Rank 0's host initialisation (coarse rigid alignment, sigma2 / beta2 guesses) is broadcast so the replicas start from the
-    same bits. Returns the solver (same result attributes as ``Morpho_pairwise``; identical on every rank)."""
+    Rank 0's inducing points and host initialisation (coarse rigid alignment, sigma2 / beta2 guesses, the SVI batch
+    permutation) are broadcast so the replicas start from the same bits whatever the ranks' NumPy random state. Returns the solver (same result attributes as ``Morpho_pairwise``; identical on
+    every rank).
+
+    Runs the full EM unless the caller passes ``SVI_mode=True`` (earlier versions replaced an explicit ``SVI_mode=True``
+    with the full EM without saying so). Under SVI every rank runs the members of each batch that fall in its block,
+    padded to one width per rank with a null column (``shard_svi_schedule``). Also supported: ``return_mapping``,
+    ``guidance_pair``, ``sparse_calculation_mode`` with ``materialize_P=True`` (one ``scipy.sparse.coo_matrix``, gathered
+    from the ranks' columns, on every rank) and ``compute_mapping``. ``K_NB``, ``P`` and ``mapping`` come back in the
+    unsharded column order. A dense ``materialize_P=True`` raises NotImplementedError, as does a pair whose block of the
+    cost matrix does not fit its GPU."""
     from .morpho_class import Morpho_pairwise
 
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0
     kw = dict(pairwise_kwargs)
     kw.setdefault("materialize_P", False)
-    kw["SVI_mode"] = False
+    kw.setdefault("SVI_mode", False)
     solver = Morpho_pairwise(sampleA=moving, sampleB=fixed, device=device, column_shard=(rank, world, mode), **kw)
+    if world > 1:  # rank 0's inducing points, so that every rank builds the same kernel matrices (U, Gamma, guidance U_I)
+        box = [solver.inducing_variables_idx if rank == 0 else None]
+        dist.broadcast_object_list(box, src=0)
+        if not np.array_equal(box[0], solver.inducing_variables_idx):
+            with torch.cuda.device(solver._dev):
+                solver._construct_kernel(box[0])
     solver.prepare_host()
     if world > 1:
         box = [{k: getattr(solver, k) for k in _HOST_INIT_FIELDS if hasattr(solver, k)} if rank == 0 else None]

@@ -195,6 +195,32 @@ def svi_chunk_schedules(sched: np.ndarray, chunks) -> list:
     return [np.ascontiguousarray(sched[:, c0:c1]) for c0, c1 in chunks]
 
 
+def shard_svi_schedule(sched: np.ndarray, n_fixed: int, rank: int, world: int):
+    """One rank's fixed-width share of the SVI schedule ``sched`` of a column-sharded pair. Returns ``(local, pos)``, both
+    [max_iter][w]: ``local[it]`` lists the members of batch ``it`` that lie in the rank's block [c0, c1) of fixed cells
+    (``column_block``), in batch order, as local column indices; ``pos[it]`` holds their positions in the batch. The rest
+    of the row is padding: the null column ``c1 - c0`` in ``local`` and -1 in ``pos``. ``w`` is the largest number of
+    members any iteration puts in the block (at least 1, so that every launch has a column), so every iteration of the
+    rank runs the same E-step launch shape."""
+    c0, c1 = (n_fixed * rank) // world, (n_fixed * (rank + 1)) // world
+    inside = (sched >= c0) & (sched < c1)
+    width = max(1, int(inside.sum(axis=1).max()))
+    local = np.full((sched.shape[0], width), c1 - c0, dtype=np.int32)
+    pos = np.full((sched.shape[0], width), -1, dtype=np.int32)
+    for it in range(sched.shape[0]):
+        members = np.flatnonzero(inside[it])
+        local[it, : members.size] = sched[it, members] - c0
+        pos[it, : members.size] = members
+    return local, pos
+
+
+# Coordinates of the null column that pads an SVI shard's iterations to one width (shard_svi_schedule). It lies so far from
+# every moving cell that build_col_lists_kernel culls it from every row block, and on the opposite side from the pad rows
+# of XAHat (+1e18), which would sit at distance 0 from a null column placed at +1e18. Its cost row is zero as well, so
+# even without culling every weight it takes part in is an exact zero.
+_NULL_COLUMN_COORD = -1e18
+
+
 def resolve_device(device) -> torch.device:
     """Reference semantics: "cpu" or a GPU index string (utils.py:35-66). Here every value maps to a CUDA device —
     there is no CPU path; ``CUDA_VISIBLE_DEVICES`` is NOT mutated (the reference does, utils.py:51)."""
@@ -317,7 +343,10 @@ class Morpho_pairwise:
     (SPB_ROW_TILE = 512 cells) and each of its four 128-cell quarters is spatially compact, and the (quarter, fixed cell) pairs
     of rows whose every pair underflows to exactly 0 in fp32 are neither read nor computed; results are bit-identical to the
     dense sweep in the same row order (all outputs are returned in the caller's row order).
-    ``column_shard`` — set by ``morpho_align_pair_sharded``: one pair's fixed cells split over several GPUs.
+    ``column_shard`` — set by ``morpho_align_pair_sharded``: one pair's fixed cells split over several GPUs. A shard runs
+    the full EM or SVI (each rank runs its members of every batch, padded with a null column), with ``return_mapping``,
+    guidance, ``sparse_calculation_mode`` and ``compute_mapping``; ``K_NB``, ``P`` (sparse COO) and ``mapping`` are gathered
+    into the unsharded column order on every rank. A dense ``materialize_P=True`` is refused (NotImplementedError).
     Cost matrix: resident ([N_B][roundup(N_A, 512)] fp32, built once) whenever the pair fits the device's free memory,
     otherwise streamed — recomputed every iteration in column chunks that fit (``cost_plan`` records which, the chunk width
     and count; ``verbose`` prints it). This is chosen from the input size and the device alone, and lets one GPU align pairs
@@ -577,13 +606,17 @@ class Morpho_pairwise:
     # ------------------------------------------------------------------------------------------------------------------
     # inducing points + kernel (morpho_class.py:825-875)
     # ------------------------------------------------------------------------------------------------------------------
-    def _construct_kernel(self):
-        uniq, uniq_idx = np.unique(self.coordsA, return_index=True, axis=0)
-        if uniq.shape[0] > self.K:
-            pick = np.random.choice(uniq.shape[0], self.K, replace=False)
-        else:
-            pick = np.arange(uniq.shape[0])
-        self.inducing_variables_idx = uniq_idx[pick]
+    def _construct_kernel(self, inducing_idx: Optional[np.ndarray] = None):
+        """Inducing points (drawn from the global ``np.random`` stream, or the moving cells ``inducing_idx`` when given) and
+        the kernel matrices built from them."""
+        if inducing_idx is None:
+            uniq, uniq_idx = np.unique(self.coordsA, return_index=True, axis=0)
+            if uniq.shape[0] > self.K:
+                pick = np.random.choice(uniq.shape[0], self.K, replace=False)
+            else:
+                pick = np.arange(uniq.shape[0])
+            inducing_idx = uniq_idx[pick]
+        self.inducing_variables_idx = np.asarray(inducing_idx)
         self.inducing_variables = self.coordsA[self.inducing_variables_idx, :]
         self.K = self.inducing_variables.shape[0]
         z = self.inducing_variables.astype(np.float64)
@@ -905,7 +938,11 @@ class Morpho_pairwise:
         if self.cost_plan.streamed:
             self._prepare_streamed_cost()
             return
-        self._GT = torch.empty((nb_loc, self.ldx), dtype=torch.float32, device=dev)
+        # an SVI shard pads its iterations to one width with the null column nb_loc: an all-zero cost row
+        self._null_column = self.column_shard is not None and self.SVI_mode
+        self._GT = torch.empty((nb_loc + int(self._null_column), self.ldx), dtype=torch.float32, device=dev)
+        if self._null_column:
+            self._GT[nb_loc:].zero_()
         gc = GeneCostBuilder(lib, dev)
         first = True
         for eA, eB, d_s, p_t, p_p in zip(
@@ -1111,11 +1148,19 @@ class Morpho_pairwise:
         f32, f64 = torch.float32, torch.float64
         c0, c1 = self._col_range()
         NB = c1 - c0  # columns held by this process (all of them unless the pair is column-sharded)
-        if self.column_shard is not None and (self.SVI_mode or self.sparse_calculation_mode or self.guidance or self.materialize_P
-                                              or self.compute_mapping or self.return_mapping):
-            raise NotImplementedError("a column-sharded pair supports the full EM only (SVI_mode=False, materialize_P=False, no "
-                                      "sparse mode / guidance / mapping outputs)")
+        if self.column_shard is not None and self.materialize_P and not self.sparse_calculation_mode:
+            raise NotImplementedError("materialize_P=True (dense) on a column-sharded pair: the N_A x N_B posterior does not fit "
+                                      "one host; use sparse_calculation_mode=True or compute_mapping=True")
+        sched = svi_schedule(self.batch_perm, self.max_iter, self.batch_size) if self.SVI_mode else None
+        self._shard_pos = None
+        self.__dict__.pop("_shard_pos_cache", None)
+        if self.SVI_mode and self.column_shard is not None:
+            # this rank's columns of every batch, padded to one width with the null column NB (_build_gene_cost)
+            sched_local, self._shard_pos = shard_svi_schedule(sched, self.NB, int(self.column_shard[0]),
+                                                              int(self.column_shard[1]))
         nbb = self.batch_size if self.SVI_mode else NB
+        if self._shard_pos is not None:
+            nbb = sched_local.shape[1]
         nbb_alloc = NB if (self.return_mapping and self.SVI_mode) else nbb
         self._NBb = nbb
         nrb = ldx // _capi.ROW_TILE
@@ -1125,8 +1170,10 @@ class Morpho_pairwise:
         s = {}
         s["xa"] = torch.zeros((3, ldx), dtype=f32, device=dev)
         s["xa"][:D, :NA] = torch.from_numpy(np.ascontiguousarray(self._sorted(self.coordsA).T, dtype=np.float32)).to(dev)
-        s["xb4"] = torch.zeros((NB, 4), dtype=f32, device=dev)
-        s["xb4"][:, :D] = torch.from_numpy(self.coordsB[c0:c1].astype(np.float32)).to(dev)
+        s["xb4"] = torch.zeros((NB + int(self._shard_pos is not None), 4), dtype=f32, device=dev)
+        s["xb4"][:NB, :D] = torch.from_numpy(self.coordsB[c0:c1].astype(np.float32)).to(dev)
+        if self._shard_pos is not None:
+            s["xb4"][NB, :3] = _NULL_COLUMN_COORD
         s["Gamma"] = torch.from_numpy(np.ascontiguousarray(self.GammaSparse, dtype=np.float32)).to(dev)
         s["kappa"] = torch.ones((ldx,), dtype=f32, device=dev)
         s["kappa"][:NA] = torch.from_numpy(self._sorted(self.kappa).astype(np.float32)).to(dev)
@@ -1175,9 +1222,8 @@ class Morpho_pairwise:
         s["trace_buf"] = torch.zeros((max(self.max_iter, 1), _capi.TRACE_STRIDE), dtype=f64, device=dev)
         s["optimal"] = torch.zeros((12,), dtype=f64, device=dev)
         if self.SVI_mode:
-            sched = svi_schedule(self.batch_perm, self.max_iter, nbb)
             self.batch_idx = sched[self.max_iter - 1].astype(np.int64) if self.max_iter > 0 else None
-            s["batch_idx"] = torch.from_numpy(sched).to(dev)
+            s["batch_idx"] = torch.from_numpy(sched if self._shard_pos is None else sched_local).to(dev)
             if self._streamed:
                 s["chunk_sched"] = [torch.from_numpy(q).to(dev) for q in svi_chunk_schedules(sched, self.cost_plan.chunks)]
         else:
@@ -1199,7 +1245,8 @@ class Morpho_pairwise:
         # params
         p = SpbEmParams()
         p.NA, p.NB, p.NBb, p.D, p.K, p.ldx = NA, NB, nbb, D, K, ldx
-        p.NB_total = self.NB if self.column_shard is not None else 0
+        # the whole iteration's column count: all fixed cells, or the SVI batch, of which this shard sees its part
+        p.NB_total = 0 if self.column_shard is None else (self.batch_size if self.SVI_mode else self.NB)
         # block partials + tickets of the ordered (reproducible) grid reductions
         n_red = max(592 * 29, ((NA + 255) // 256) * 4, 320 * K * (K + 3) if K <= 32 else 0) + 64
         s["red_scratch"] = torch.zeros((n_red,), dtype=f64, device=dev)
@@ -1330,24 +1377,96 @@ class Morpho_pairwise:
         p.rowstat = buf.data_ptr()
         p.shard_flags = buf.data_ptr() + n_stat * 8
 
-    def _shard_row_statistics(self, st):
-        """Row statistics of a column-sharded pair: local fold, sum over the ranks, finish (replaces spb_row_finalize)."""
-        import torch.distributed as dist
-
-        lib, p, s = self._lib, self._params, self._state
+    def _shard_fold(self, st) -> torch.Tensor:
+        """Column-sharded pair: fold this rank's row partials of the E-step into the fp64 row statistics; returns the view
+        that the ranks sum."""
         parity = self._shard_epoch & 1
         self._shard_epoch += 1
-        check(lib.spb_row_fold(C.byref(p), parity, st), "spb_row_fold")
+        check(self._lib.spb_row_fold(C.byref(self._params), parity, st), "spb_row_fold")
+        return self._state["rowstat"][parity * 8 * self.ldx : (parity + 1) * 8 * self.ldx]
+
+    def _shard_sum(self, view: torch.Tensor, st):
+        """Sum the view of ``_shard_fold`` over the ranks, in place. ``p2p``: one kernel reads the peers' views over NVLink
+        in rank order and also finishes the row statistics."""
         if self._shard_mode == "p2p":
-            check(lib.spb_row_stats_p2p(C.byref(p), parity, self._shard_epoch, st), "spb_row_stats_p2p")
+            check(self._lib.spb_row_stats_p2p(C.byref(self._params), (self._shard_epoch - 1) & 1, self._shard_epoch, st),
+                  "spb_row_stats_p2p")
+            return
+        comm = getattr(self, "_shard_comm", None)
+        if comm is not None:  # tests: several shards of one process, each driven by its own thread
+            comm.sum_(self, view)
         else:
-            view = s["rowstat"][parity * 8 * self.ldx : (parity + 1) * 8 * self.ldx]
-            hook = getattr(self, "_shard_reduce_hook", None)
-            if hook is not None:  # tests: several shards stepped in lock-step inside one process
-                hook(self, view)
-            elif dist.is_initialized() and dist.get_world_size() > 1:
+            import torch.distributed as dist
+
+            if dist.is_initialized() and dist.get_world_size() > 1:
                 dist.all_reduce(view)
-            check(lib.spb_row_stats_finalize(C.byref(p), parity, st), "spb_row_stats_finalize")
+
+    def _shard_finish_rows(self, st):
+        """Finish the row statistics from the view of ``_shard_fold`` once ``_shard_sum`` made it the sum over the ranks
+        (``p2p``: already finished by ``_shard_sum``)."""
+        if self._shard_mode == "p2p":
+            return
+        check(self._lib.spb_row_stats_finalize(C.byref(self._params), (self._shard_epoch - 1) & 1, st),
+              "spb_row_stats_finalize")
+
+    def _shard_row_statistics(self, st):
+        """Row statistics of a column-sharded pair: local fold, sum over the ranks, finish (replaces spb_row_finalize)."""
+        self._shard_sum(self._shard_fold(st), st)
+        self._shard_finish_rows(st)
+
+    def _shard_gather(self, t: torch.Tensor) -> list:
+        """Every rank's ``t`` (per-column rows of its E-step columns), in rank order; only this rank's own without a
+        process group."""
+        comm = getattr(self, "_shard_comm", None)
+        if comm is not None:
+            return comm.gather(self, t)
+        import torch.distributed as dist
+
+        if dist.is_initialized() and dist.get_world_size() > 1:
+            from .distributed import all_gather_rows
+
+            return all_gather_rows(t)
+        return [t]
+
+    def _shard_max_(self, keys: torch.Tensor) -> torch.Tensor:
+        """In place: the element-wise maximum of every rank's int64 ``keys`` (argmax keys of non-negative values)."""
+        comm = getattr(self, "_shard_comm", None)
+        if comm is not None:
+            comm.max_(self, keys)
+        else:
+            import torch.distributed as dist
+
+            if dist.is_initialized() and dist.get_world_size() > 1:
+                dist.all_reduce(keys, op=dist.ReduceOp.MAX)
+        return keys
+
+    def _shard_positions(self) -> list:
+        """Output column of every E-step column of every rank, in rank order (-1: null column): batch positions for an SVI
+        E-step, fixed cells for a full one."""
+        from .distributed import column_block
+
+        world, svi = int(self.column_shard[1]), bool(self._params.svi)
+        cache = self.__dict__.setdefault("_shard_pos_cache", {})
+        if svi not in cache:
+            if svi:
+                sched = svi_schedule(self.batch_perm, self.max_iter, self.batch_size)
+                it = max(self.max_iter - 1, 0)
+                cache[svi] = [shard_svi_schedule(sched, self.NB, r, world)[1][it] for r in range(world)]
+            else:
+                cache[svi] = [np.arange(*column_block(self.NB, r, world), dtype=np.int32) for r in range(world)]
+        return cache[svi]
+
+    def _shard_columns(self, t: torch.Tensor, n_out: int, fill=0) -> np.ndarray:
+        """Per-column rows ``t`` [NBb, ...] of every rank's last E-step, assembled on the host in the unsharded column order
+        ([n_out, ...]; null columns dropped). Without a process group only this rank's columns are returned."""
+        from .distributed import assemble_columns
+
+        parts = [q.cpu().numpy() for q in self._shard_gather(t)]
+        pos = self._shard_positions()
+        if len(parts) == 1 and len(pos) > 1:  # no collective: this rank's own columns
+            mine = pos[int(self.column_shard[0])]
+            return parts[0][: mine.shape[0]][mine >= 0]
+        return assemble_columns(parts, pos, n_out, fill)
 
     def _pinv_eps(self) -> float:
         """Machine epsilon behind scipy.linalg.pinv's default cutoff in the reference (utils.py:1435): float32 for the
@@ -1402,12 +1521,40 @@ class Morpho_pairwise:
         if not (large_K or capture_P or sweep_events is not None or self.column_shard is not None or self._streamed):
             check(lib.spb_em_iteration(C.byref(p), it, st), "spb_em_iteration")
             return
+        if self.column_shard is not None:  # (a column-sharded pair is never streamed)
+            view = self._shard_iteration_local(it, st, capture_P, sweep_events)
+            self._shard_sum(view, st)
+            self._shard_iteration_finish(it, st)
+            return
         if self._streamed:
             self._estep_only(it, st, on_chunk=self._streamed_capture() if capture_P else None)
         else:
             self._estep_only(it, st, sweep_events)
             if capture_P:
                 self._capture_P(it, st)
+        self._mstep(it, st)
+
+    def _shard_iteration_local(self, it: int, st, capture_P: bool = False,
+                               sweep_events: Optional[list] = None) -> torch.Tensor:
+        """First half of a column-sharded iteration: the E-step of this rank's columns (and the posterior capture of the
+        last iteration) up to the fold of its row statistics. Returns the fp64 view that ``_shard_sum`` sums over the ranks
+        before ``_shard_iteration_finish`` (``_iteration`` runs the three in this order)."""
+        self._estep_local(it, st, sweep_events)
+        if capture_P:
+            self._capture_P(it, st)
+        return self._shard_fold(st)
+
+    def _shard_iteration_finish(self, it: int, st):
+        """Second half of a column-sharded iteration, once ``_shard_sum`` made the view of ``_shard_iteration_local`` the sum
+        over the ranks: finish the row statistics, then the replicated M-step."""
+        self._shard_finish_rows(st)
+        self._mstep(it, st)
+
+    def _mstep(self, it: int, st):
+        """The M-step of one iteration (split path of ``_iteration``)."""
+        lib, p = self._lib, self._params
+        nonrigid = it > self.nonrigid_start_iter
+        large_K = nonrigid and self.K > _capi.MAX_K_FUSED
         check(lib.spb_update_gamma_alpha(C.byref(p), st), "spb_update_gamma_alpha")
         if nonrigid:
             check(lib.spb_nonrigid_accumulate(C.byref(p), st), "spb_nonrigid_accumulate")
@@ -1429,7 +1576,11 @@ class Morpho_pairwise:
         if self.compute_mapping:  # row / column maxima of the same posterior, straight from the cost matrix
             self._rowbest = torch.zeros((self.NA,), dtype=torch.int64, device=self._dev)
             self._colbest = torch.zeros((self._NBb,), dtype=torch.int64, device=self._dev)
-            check(lib.spb_posterior_argmax(C.byref(p), it, ptr(self._rowbest), ptr(self._colbest), st), "spb_posterior_argmax")
+            colmap = None
+            if self.column_shard is not None:  # row keys carry the unsharded column index; null columns are skipped
+                colmap = torch.from_numpy(self._shard_positions()[int(self.column_shard[0])]).to(self._dev)
+            check(lib.spb_posterior_argmax_mapped(C.byref(p), it, ptr(colmap), ptr(self._rowbest), ptr(self._colbest), st),
+                  "spb_posterior_argmax_mapped")
         if not self.materialize_P:
             self._P_dev = "skipped"
             return
@@ -1443,26 +1594,38 @@ class Morpho_pairwise:
             self._P_dev = torch.empty((self.NA, self._NBb), dtype=torch.float32, device=self._dev)
             check(lib.spb_materialize_P(C.byref(p), it, ptr(self._P_dev), self._NBb, st), "spb_materialize_P")
 
-    def _sparse_P_to_coo(self, dt):
-        """scipy COO in the reference's layout (utils.py:1385-1392,1506-1510): per column the k entries in descending
-        order, columns concatenated."""
+    def _sparse_P_to_coo(self, dt, P_rows: Optional[torch.Tensor] = None, P_vals: Optional[torch.Tensor] = None):
+        """scipy COO in the reference's layout (utils.py:1385-1392,1506-1510) from the [n_cols][sparse_top_k] entries of
+        ``spb_sparse_P_emit`` (default: this solver's last capture): per column the k entries in descending order, columns
+        concatenated."""
         import scipy.sparse as sp
 
+        P_rows = self._P_rows if P_rows is None else P_rows
+        P_vals = self._P_vals if P_vals is None else P_vals
+
         k = min(int(self.sparse_top_k), self.NA)
-        vals, order = torch.sort(self._P_vals[:, :k], dim=1, descending=True, stable=True)
-        rows = torch.gather(self._P_rows[:, :k].long(), 1, order).cpu().numpy()
+        n_cols = P_rows.shape[0]
+        vals, order = torch.sort(P_vals[:, :k], dim=1, descending=True, stable=True)
+        rows = torch.gather(P_rows[:, :k].long(), 1, order).cpu().numpy()
         if self._perm is not None:
             rows = self._perm[rows]
-        col = np.repeat(np.arange(self._NBb), k)
-        return sp.coo_matrix((vals.cpu().numpy().astype(dt).reshape(-1), (rows.reshape(-1), col)),
-                             shape=(self.NA, self._NBb))
+        col = np.repeat(np.arange(n_cols), k)
+        return sp.coo_matrix((vals.cpu().numpy().astype(dt).reshape(-1), (rows.reshape(-1), col)), shape=(self.NA, n_cols))
 
     def _estep_only(self, it: int, st, sweep_events: Optional[list] = None, on_chunk=None):
         """One E-step + the statistics the closing similarity needs (used for return_mapping under SVI)."""
-        lib, p = self._lib, self._params
         if self._streamed:
             self._estep_streamed(it, st, on_chunk)
             return
+        self._estep_local(it, st, sweep_events)
+        if self.column_shard is not None:
+            self._shard_row_statistics(st)
+        else:
+            check(self._lib.spb_row_finalize(C.byref(self._params), st), "spb_row_finalize")
+
+    def _estep_local(self, it: int, st, sweep_events: Optional[list] = None):
+        """The E-step of a resident cost matrix up to its row partials (sweep 2)."""
+        lib, p = self._lib, self._params
         check(lib.spb_iter_begin(C.byref(p), it, st), "spb_iter_begin")
         check(lib.spb_gather_cols(C.byref(p), it, st), "spb_gather_cols")
         check(lib.spb_estep_col_lists(C.byref(p), st), "spb_estep_col_lists")
@@ -1481,10 +1644,6 @@ class Morpho_pairwise:
         if sweep_events is not None:
             e3.record()
             sweep_events.append((e0, e1, e2, e3))
-        if self.column_shard is not None:
-            self._shard_row_statistics(st)
-        else:
-            check(lib.spb_row_finalize(C.byref(p), st), "spb_row_finalize")
 
     def _chunk_params(self, k: int, c0: int, c1: int) -> SpbEmParams:
         """Parameters of one column chunk [c0, c1) of the E-step that ``_params`` describes: its columns are fixed cells
@@ -1709,11 +1868,14 @@ class Morpho_pairwise:
         if full_mapping:
             # full (non-SVI) posterior with the final parameters (morpho_class.py:300-302)
             self.SVI_mode = False
-            p.svi, p.NBb = 0, self.NB
+            nb = self._col_range()[1] - self._col_range()[0]  # a shard's closing E-step covers its whole block
+            p.svi, p.NBb = 0, nb
+            if self.column_shard is not None:
+                p.NB_total = self.NB
             if not self._streamed:  # streamed: the column segments stay those of the chunk width
-                p.seg1 = p.seg2 = self._choose_segments(self.ldx // _capi.ROW_TILE, self.NB,
+                p.seg1 = p.seg2 = self._choose_segments(self.ldx // _capi.ROW_TILE, nb,
                                                         torch.cuda.get_device_properties(self._dev).multi_processor_count)
-            self._NBb = self.NB
+            self._NBb = nb
             self._estep_only(last_iter, st, on_chunk=capture())
             # scalar Sp's must become the un-averaged sums (morpho_class.py:1183-1185)
             sc = self._read_scalars()
@@ -1747,19 +1909,12 @@ class Morpho_pairwise:
         self.XAHat, self.RnA, self.VnA = rows("XAHat"), rows("RnA"), rows("VnA")
         self.optimal_RnA = (self.coordsA.astype(np.float64) @ self.optimal_R.astype(np.float64).T + self.optimal_t).astype(dt)
         self.K_NA = vec("K_NA")
-        self.K_NB = s["K_NB"][: self._NBb].cpu().numpy().astype(dt)
-        if self.column_shard is not None:  # every rank holds the column sums of its own block of fixed cells
-            import torch.distributed as dist
-
-            if dist.is_initialized() and dist.get_world_size() > 1:
-                world = dist.get_world_size()
-                width = (self.NB + world - 1) // world + 1
-                mine = torch.zeros((width,), dtype=torch.float32, device=self._dev)
-                mine[: self._NBb] = s["K_NB"][: self._NBb]
-                parts = [torch.zeros_like(mine) for _ in range(world)]
-                dist.all_gather(parts, mine)
-                sizes = [(self.NB * (r + 1)) // world - (self.NB * r) // world for r in range(world)]
-                self.K_NB = np.concatenate([q[:n].cpu().numpy() for q, n in zip(parts, sizes)]).astype(dt)
+        # the unsharded column count of the last E-step: the SVI batch or all fixed cells
+        n_cols = self.batch_size if self._params.svi else self.NB
+        if self.column_shard is None:
+            self.K_NB = s["K_NB"][: self._NBb].cpu().numpy().astype(dt)
+        else:  # every rank holds the column sums of its own columns: gathered into the unsharded order
+            self.K_NB = self._shard_columns(s["K_NB"][: self._NBb], n_cols).astype(dt)
         self.K_NA_spatial = vec("K_NA_spatial")
         self.K_NA_sigma2 = vec("K_NA_sigma2")
         self.alpha = vec("alpha")
@@ -1775,15 +1930,23 @@ class Morpho_pairwise:
         if self.compute_mapping:
             from .mapping import ArgmaxPi
 
-            ra, rv = ArgmaxPi.decode(self._rowbest.cpu().numpy().view(np.uint64))
-            ca, cv = ArgmaxPi.decode(self._colbest.cpu().numpy().view(np.uint64))
+            rowbest, colbest = self._rowbest.cpu().numpy(), self._colbest.cpu().numpy()
+            if self.column_shard is not None:  # row keys: the largest over the ranks; column keys: gathered
+                rowbest = self._shard_max_(self._rowbest).cpu().numpy()
+                colbest = self._shard_columns(self._colbest, n_cols)
+            ra, rv = ArgmaxPi.decode(rowbest.view(np.uint64))
+            ca, cv = ArgmaxPi.decode(colbest.view(np.uint64))
             if self._perm is not None:  # device rows are in processing order
                 ra, rv, ca = self._unsorted(ra), self._unsorted(rv), self._perm[ca]
-            self.mapping = ArgmaxPi((NA, self._NBb), ra, rv.astype(dt), ca, cv.astype(dt))
+            self.mapping = ArgmaxPi((NA, colbest.shape[0]), ra, rv.astype(dt), ca, cv.astype(dt))
             self._rowbest = self._colbest = None
         if self.materialize_P:
             if self.sparse_calculation_mode:
-                self.P = self._sparse_P_to_coo(dt)
+                rows, vals = self._P_rows, self._P_vals
+                if self.column_shard is not None:  # every rank emitted the entries of its own columns
+                    rows = torch.from_numpy(self._shard_columns(rows, n_cols))
+                    vals = torch.from_numpy(self._shard_columns(vals, n_cols))
+                self.P = self._sparse_P_to_coo(dt, rows, vals)
                 self._P_rows = self._P_vals = None
             else:
                 _count_d2h(self._P_dev)

@@ -1249,11 +1249,14 @@ col_argmax_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __re
   }
 }
 
-// one thread per moving cell, blockIdx.y = column segment; partial results are merged with a 64-bit atomicMax
+// one thread per moving cell, blockIdx.y = column segment; partial results are merged with a 64-bit atomicMax.
+// colmap (optional): output column index of every launch position, -1 = no column (skipped); without it the key carries j.
+// A column-sharded pair passes its block's global column indices, so the ranks' keys merge with a plain maximum.
 __global__ void __launch_bounds__(256)
 row_argmax_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __restrict__ batch_base,
                   const float* __restrict__ colconst, const float* __restrict__ XA, const float* __restrict__ lm,
-                  const spb_scalars* __restrict__ sc, int NA, int NBb, unsigned long long* __restrict__ rowbest) {
+                  const spb_scalars* __restrict__ sc, int NA, int NBb, const int32_t* __restrict__ colmap,
+                  unsigned long long* __restrict__ rowbest) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= NA) return;
   const int per = (NBb + gridDim.y - 1) / gridDim.y;
@@ -1262,13 +1265,15 @@ row_argmax_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __re
   const int32_t* col_index = batch_cols(batch_base, sc, NBb);
   unsigned long long best = 0ull;
   for (int j = j0; j < j1; ++j) {
+    const int jo = colmap ? colmap[j] : j;
+    if (jo < 0) continue;
     const float4 c0 = *reinterpret_cast<const float4*>(colconst + (int64_t)j * SPB_COLCONST_FLOATS);
     const float4 c1 = *reinterpret_cast<const float4*>(colconst + (int64_t)j * SPB_COLCONST_FLOATS + 4);
     const float cj = colconst[(int64_t)j * SPB_COLCONST_FLOATS + 10];
     const int64_t row = col_index ? (int64_t)col_index[j] : (int64_t)j;
     float w = pair_weight(x0, x1, x2, c0.x, c0.z, c1.x, cq, li, GT[row * ldx + i]);
     w = w >= colconst[(int64_t)j * SPB_COLCONST_FLOATS + 18] ? w : 0.f;  // sparse mode: entries below the column's top-k are absent
-    const unsigned long long key = argmax_key(w * cj, j);
+    const unsigned long long key = argmax_key(w * cj, jo);
     best = key > best ? key : best;
   }
   if (j0 < j1) atomicMax(rowbest + i, best);
@@ -1412,6 +1417,11 @@ extern "C" int spb_sparse_P_emit(const spb_em_params* p, int32_t iter, int32_t* 
 
 extern "C" int spb_posterior_argmax(const spb_em_params* p, int32_t iter, uint64_t* rowbest, uint64_t* colbest,
                                     void* stream) {
+  return spb_posterior_argmax_mapped(p, iter, nullptr, rowbest, colbest, stream);
+}
+
+extern "C" int spb_posterior_argmax_mapped(const spb_em_params* p, int32_t iter, const int32_t* colmap, uint64_t* rowbest,
+                                           uint64_t* colbest, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (colbest) {
     col_argmax_kernel<<<p->NBb, kSelThreads, 0, st>>>(p->GT, p->ldx, gt_batch_ptr(p, iter), p->colconst, p->XAHat, p->lm,
@@ -1425,7 +1435,7 @@ extern "C" int spb_posterior_argmax(const spb_em_params* p, int32_t iter, uint64
     int nseg = (spb_num_sms() * 8 + nrow - 1) / nrow;  // ~8 CTAs per SM
     nseg = nseg < 1 ? 1 : (nseg > p->NBb ? p->NBb : nseg);
     row_argmax_kernel<<<dim3(nrow, nseg), 256, 0, st>>>(p->GT, p->ldx, gt_batch_ptr(p, iter), p->colconst, p->XAHat, p->lm,
-                                                        p->sc, p->NA, p->NBb, (unsigned long long*)rowbest);
+                                                        p->sc, p->NA, p->NBb, colmap, (unsigned long long*)rowbest);
     SPB_CHECK_LAUNCH();
   }
   return 0;
