@@ -7,6 +7,9 @@ set -u
 TOOL=${1:-all}
 WIDE="(test_full_run_matches_reference and 2d_full]) or (test_sparse_estep_matches_float64_oracle and 0]) or (test_voxel_data_device_matches_host and 2-float32) or test_gene_cost_kl_matches_oracle or (test_kwargs_surface and large_K)"
 NARROW="(test_single_estep_matches_float64_oracle and 2d_full and 0-) or (test_sparse_estep_matches_float64_oracle and 0]) or test_gene_cost_kl_matches_oracle"
+# M-step kernels: the Jacobi solve (shared memory, block barriers), the low-rank apply, the ordered moment reduction
+MSTEP="(spectrum_and_warm_starts and cutoff_straddle) or lowrank or rigid_moments or (one_mstep and (K65 or K33))"
+JACOBI="spectrum_and_warm_starts and (clustered-15 or cutoff_straddle-64) or svi_blend_and_guidance"
 run() {  # tool, pytest args...
   local tool=$1; shift
   echo "=== compute-sanitizer --tool $tool : $*"
@@ -18,12 +21,15 @@ if [ "$TOOL" = memcheck ] || [ "$TOOL" = all ]; then
   run memcheck tests/test_gpu_gram.py -k "64-7000 or 257-4100 or 15-5000 or 3-900"
   run memcheck tests/test_gpu_shard.py -k "1]"
   run memcheck tests/test_gpu_shard_options.py -k "mapping_from_identical_state or svi_estep_from_identical_state"
+  run memcheck tests/test_gpu_mstep.py -k "$MSTEP"
 fi
 if [ "$TOOL" = racecheck ] || [ "$TOOL" = all ]; then
   run racecheck tests/test_gpu_parity.py -k "$NARROW"
   run racecheck tests/test_gpu_gram.py -k "64-7000"
+  run racecheck tests/test_gpu_mstep.py -k "$JACOBI"
 fi
 if [ "$TOOL" = synccheck ] || [ "$TOOL" = all ]; then
   run synccheck tests/test_gpu_parity.py -k "$NARROW"
   run synccheck tests/test_gpu_gram.py -k "64-7000"
+  run synccheck tests/test_gpu_mstep.py -k "$JACOBI"
 fi

@@ -474,9 +474,12 @@ __global__ void __launch_bounds__(256) nonrigid_solve_kernel(spb_em_params p) {
   __syncthreads();
   for (int q = tid; q < K * K; q += nt) {
     const int r = q / K, c = q % K;
-    double s = 0;
-    for (int e = 0; e < Kp; ++e) s += V[r * Kp + e] * cs[e] * V[c * Kp + e];
-    p.Sigma[q] = s;
+    if (r <= c) {  // upper triangle, mirrored: Sigma is exactly symmetric like SigmaInv
+      double s = 0;
+      for (int e = 0; e < Kp; ++e) s += V[r * Kp + e] * cs[e] * V[c * Kp + e];
+      p.Sigma[q] = s;
+      p.Sigma[c * K + r] = s;
+    }
     if (ws != nullptr) ws[1 + q] = V[r * Kp + c];  // eigenbasis for the next iteration's warm start
   }
   if (ws != nullptr && tid == 0) ws[0] = (double)K;
