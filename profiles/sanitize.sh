@@ -10,6 +10,9 @@ NARROW="(test_single_estep_matches_float64_oracle and 2d_full and 0-) or (test_s
 # M-step kernels: the Jacobi solve (shared memory, block barriers), the low-rank apply, the ordered moment reduction
 MSTEP="(spectrum_and_warm_starts and cutoff_straddle) or lowrank or rigid_moments or (one_mstep and (K65 or K33))"
 JACOBI="spectrum_and_warm_starts and (clustered-15 or cutoff_straddle-64) or svi_blend_and_guidance"
+# sparse top-k select: candidate-cap overflow, ties at tau, subnormals (racecheck / synccheck); 514 row blocks (memcheck)
+SELECT="test_written_cap_ties_subnormals_against_replay and 1024-True"
+MASKOFF="test_mask_off_above_512_row_blocks and 32"
 run() {  # tool, pytest args...
   local tool=$1; shift
   echo "=== compute-sanitizer --tool $tool : $*"
@@ -22,14 +25,17 @@ if [ "$TOOL" = memcheck ] || [ "$TOOL" = all ]; then
   run memcheck tests/test_gpu_shard.py -k "1]"
   run memcheck tests/test_gpu_shard_options.py -k "mapping_from_identical_state or svi_estep_from_identical_state"
   run memcheck tests/test_gpu_mstep.py -k "$MSTEP"
+  run memcheck tests/test_gpu_posterior_select.py -k "$MASKOFF"
 fi
 if [ "$TOOL" = racecheck ] || [ "$TOOL" = all ]; then
   run racecheck tests/test_gpu_parity.py -k "$NARROW"
   run racecheck tests/test_gpu_gram.py -k "64-7000"
   run racecheck tests/test_gpu_mstep.py -k "$JACOBI"
+  run racecheck tests/test_gpu_posterior_select.py -k "$SELECT"
 fi
 if [ "$TOOL" = synccheck ] || [ "$TOOL" = all ]; then
   run synccheck tests/test_gpu_parity.py -k "$NARROW"
   run synccheck tests/test_gpu_gram.py -k "64-7000"
   run synccheck tests/test_gpu_mstep.py -k "$JACOBI"
+  run synccheck tests/test_gpu_posterior_select.py -k "$SELECT"
 fi

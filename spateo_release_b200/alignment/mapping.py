@@ -27,7 +27,8 @@ class ArgmaxPi:
 
     Tie-breaking differs from the reference for equal NON-ZERO maxima (exact duplicates: cells with identical coordinates
     and expression): ``get_optimal_mapping_relationship`` (spateo/alignment/utils.py:157-191) resolves such ties with a
-    KD-tree over the coordinates, here the lowest index in the solver's processing (Morton) order wins. Ties at value 0
+    KD-tree over the coordinates. Here a row's tie goes to the lowest column index, and a column's tie to the moving cell that
+    comes first in the solver's processing order (the k-d order of ``kd_order``), not the lowest input index. Ties at value 0
     (rows / columns without any posterior mass) are handled like the reference. Pass a dense ``pi`` to get the reference's
     tie rule."""
 

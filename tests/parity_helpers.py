@@ -272,3 +272,134 @@ def device_rows(m, name):
 
 def device_pxb(m):
     return m._unsorted(m._state["PXB"][: m.D, : m.NA].T.contiguous().cpu().numpy())
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The sparse top-k posterior and the posterior argmax
+# ---------------------------------------------------------------------------------------------------------------------
+def replay_weights(m, it, q=None):
+    """The device's own pair weights w = q g, [N_A, NBb] float32 in DEVICE row order, for the E-step that has just run
+    (``q``: the parameters of one streamed column chunk; default the solver's). ``spb_materialize_P`` writes
+    ex2(c_q d + lm) * g * c_j; with every c_j replaced by 1.0 the last product is exact and it writes w itself."""
+    import torch
+
+    from spateo_release_b200._capi import SpbEmParams, check, ptr
+
+    p = SpbEmParams.from_buffer_copy(m._params if q is None else q)
+    cc = m._state["colconst"].clone()
+    cc[:, 10] = 1.0
+    p.colconst = cc.data_ptr()
+    W = torch.empty((m.NA, p.NBb), dtype=torch.float32, device=m._dev)
+    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    check(m._lib.spb_materialize_P(C.byref(p), it, ptr(W), p.NBb, st), "spb_materialize_P")
+    torch.cuda.synchronize()
+    return W.cpu().numpy()
+
+
+def topk_replay(W, k, c, Y=None, block=1024):
+    """What the sparse top-k kernels compute from the weights ``W`` [N_A, NB] (float32), the column factors ``c`` [NB]
+    (float32) and the fixed coordinates ``Y`` [NB, D]:
+      tau        per column the k-th largest w (k clamped to N_A), 0 when the column has fewer non-zero weights (float32)
+      n_above    number of w > tau; n_ties: number of w == tau (tau > 0), else 0
+      K_NB       c_j * sum_{w >= tau} w in fp64 (every copy of tau counts)
+      K_NB_k     c_j * (sum of exactly k entries: every w > tau, then ties at tau) in fp64, the reference's column sum
+      K_NA, PXB  the row sums sweep 2 forms, sum_j c_j w_ij [w_ij >= tau_j] and the same weighted by y_j (fp64)."""
+    W = np.asarray(W, dtype=np.float32)
+    NA, NB = W.shape
+    kk = min(int(k), NA)
+    c64 = np.asarray(c, np.float64)
+    out = dict(tau=np.zeros(NB, np.float32), n_above=np.zeros(NB, np.int64), n_ties=np.zeros(NB, np.int64),
+               K_NB=np.zeros(NB), K_NB_k=np.zeros(NB), K_NA=np.zeros(NA))
+    if Y is not None:
+        out["PXB"] = np.zeros((NA, np.shape(Y)[1]))
+    for j0 in range(0, NB, block):  # column blocks bound the fp64 temporaries
+        j1 = min(NB, j0 + block)
+        Wb = W[:, j0:j1]
+        tau = -np.partition(-Wb, kk - 1, axis=0)[kk - 1]
+        tau = np.where(tau > 0, tau, np.float32(0)).astype(np.float32)
+        kept = np.where(Wb >= tau[None, :], Wb.astype(np.float64), 0.0)
+        above = Wb > tau[None, :]
+        n_above = above.sum(0)
+        n_ties = np.where(tau > 0, (Wb == tau[None, :]).sum(0), 0)
+        mass_above = np.where(above, kept, 0.0).sum(0)
+        out["tau"][j0:j1], out["n_above"][j0:j1], out["n_ties"][j0:j1] = tau, n_above, n_ties
+        out["K_NB"][j0:j1] = c64[j0:j1] * kept.sum(0)
+        out["K_NB_k"][j0:j1] = c64[j0:j1] * (mass_above + np.minimum(n_ties, kk - n_above) * tau.astype(np.float64))
+        out["K_NA"] += kept @ c64[j0:j1]
+        if Y is not None:
+            out["PXB"] += kept @ (c64[j0:j1, None] * np.asarray(Y, np.float64)[j0:j1])
+    return out
+
+
+def argmax_keys(v, idx):
+    """64-bit argmax keys of ``row_argmax`` / ``col_argmax``: the float bits of the value above the complemented index, so
+    the unsigned maximum is the largest value and, among equal values, the lowest index."""
+    v = np.ascontiguousarray(v, dtype=np.float32)
+    return (v.view(np.uint32).astype(np.uint64) << np.uint64(32)) | (np.uint64(0xFFFFFFFF) - np.asarray(idx).astype(np.uint64))
+
+
+def argmax_replay(W, c, tau, colmap=None, block=64):
+    """Row and column argmax keys of the posterior P = w c (fp32 products) from the weights ``W`` [N_A, NB] (device row
+    order): a row's key skips entries below their column's ``tau`` (sparse mode; tau = 0 keeps all) and carries the column
+    index ``colmap[j]`` (-1: column skipped; default j); a column's key carries the device row index."""
+    W = np.asarray(W, dtype=np.float32)
+    NA, NB = W.shape
+    c = np.asarray(c, dtype=np.float32)
+    colmap = np.arange(NB) if colmap is None else np.asarray(colmap)
+    rowkey = np.zeros(NA, dtype=np.uint64)
+    colkey = np.zeros(NB, dtype=np.uint64)
+    rows = np.arange(NA)
+    for j0 in range(0, NB, block):
+        j1 = min(NB, j0 + block)
+        P = W[:, j0:j1] * c[None, j0:j1]
+        ck = argmax_keys(P, rows[:, None]).max(0)
+        colkey[j0:j1] = ck
+        live = colmap[j0:j1] >= 0
+        if live.any():
+            Ps = np.where(W[:, j0:j1] >= tau[None, j0:j1], W[:, j0:j1], np.float32(0)) * c[None, j0:j1]
+            rk = argmax_keys(Ps[:, live], colmap[j0:j1][live][None, :]).max(1)
+            rowkey = np.maximum(rowkey, rk)
+    return rowkey, colkey
+
+
+def sparse_posterior_reference(Dim, XAHat, YB, G, sigma2, model_mul, gamma, samples_s, sigma2_variance, ks, chunk=1000,
+                               dtype=np.float64):
+    """``get_P_core`` followed by ``dense_to_sparse_topk`` on a given cost matrix ``G`` [N_A, NB] (the product of the
+    expression terms, passed as a "prob" term), evaluated in column chunks: every normalisation and the top-k are per
+    column. For each k in ``ks``: the COO entries ``rows`` / ``vals`` [NB, k] (descending within a column), the row sums
+    K_NA, the column sums K_NB, P @ YB, and each column's k-th and (k+1)-th largest values (``kth``, ``kth1``; 0 past N_A).
+    ``dtype=np.float32`` restates it in fp32 (the scale of what an fp32 evaluation of the reference computes)."""
+    from oracle.morpho_oracle import get_P_core
+
+    f = lambda a: np.asarray(a, dtype=dtype)
+    XAHat, YB, G, model_mul = f(XAHat), f(YB), np.asarray(G), f(model_mul)
+    NA, NB = G.shape
+    ks = [int(k) for k in ks]
+    out = {k: dict(rows=np.zeros((NB, min(k, NA)), np.int64), vals=np.zeros((NB, min(k, NA)), dtype), K_NA=np.zeros(NA, dtype),
+                   K_NB=np.zeros(NB, dtype), PXB=np.zeros((NA, YB.shape[1]), dtype), kth=np.zeros(NB, dtype),
+                   kth1=np.zeros(NB, dtype)) for k in ks}
+    top = min(max(ks) + 1, NA)
+    for j0 in range(0, NB, chunk):
+        j1 = min(NB, j0 + chunk)
+        spatial = ((XAHat[:, None, :] - YB[None, j0:j1, :]) ** 2).sum(-1)
+        P, _, _, _ = get_P_core(Dim=Dim, spatial_dist=spatial, exp_dist=[f(G[:, j0:j1])], sigma2=sigma2, model_mul=model_mul,
+                                gamma=gamma, samples_s=samples_s, sigma2_variance=sigma2_variance, probability_type=["prob"])
+        P = f(P)
+        # descending with the lowest row first among equal values, like the reference's stable argsort of -P
+        part = np.argpartition(-P, top - 1, axis=0)[:top] if top < NA else np.broadcast_to(np.arange(NA)[:, None], P.shape)
+        pv = np.take_along_axis(P, part, axis=0)
+        order = np.lexsort((part, -pv), axis=0)
+        idx, val = np.take_along_axis(part, order, axis=0), np.take_along_axis(pv, order, axis=0)
+        for k in ks:
+            kk = min(k, NA)
+            o = out[k]
+            o["rows"][j0:j1], o["vals"][j0:j1] = idx[:kk].T, val[:kk].T
+            o["kth"][j0:j1] = val[kk - 1]
+            if kk < NA:
+                o["kth1"][j0:j1] = val[kk]
+            Ps = np.zeros_like(P)
+            np.put_along_axis(Ps, idx[:kk], val[:kk], axis=0)
+            o["K_NA"] += Ps.sum(1)
+            o["K_NB"][j0:j1] = Ps.sum(0)
+            o["PXB"] += Ps @ YB[j0:j1]
+    return out
