@@ -34,6 +34,7 @@ extern "C" {
 #define SPB_MAX_K_FUSED 64 /* largest K solved by the in-library Jacobi kernel */
 #define SPB_TRACE_STRIDE 8
 #define SPB_COLMASK_WORDS 16 /* per-column bit mask over row blocks (sparse mode): up to 512 row blocks = 262,144 rows */
+#define SPB_TRANSFER_PANEL 16 /* features per pass of the posterior-transfer kernels */
 
 #define SPB_EINVAL (-2)
 #define SPB_EUNSUPPORTED (-3)
@@ -265,6 +266,18 @@ int spb_posterior_argmax(const spb_em_params* p, int32_t iter, uint64_t* rowbest
 int spb_posterior_argmax_mapped(const spb_em_params* p, int32_t iter, const int32_t* colmap, uint64_t* rowbest,
                                 uint64_t* colbest, void* stream);
 int spb_materialize_P(const spb_em_params* p, int32_t iter, float* P, int64_t ldp, void* stream); /* utils.py:1083 */
+/* Posterior transfer of the last E-step without forming P (sparse mode: the entries w >= tau_j, as sweep 2 keeps them).
+   Both visit the tiles and quarters of the E-step's work lists, SPB_TRANSFER_PANEL features per pass, no float atomics.
+   rows: out[f][i] (fp64, [ldf][ldx], processing order) = (P @ F_B)[i][f] for f < F; F_B is [rows of xb4][ldf] (fixed
+         cells, ldf a multiple of SPB_TRANSFER_PANEL, pad features zero); part: [seg2][SPB_TRANSFER_PANEL][ldx] floats.
+         The segment partials are folded in fp64 in segment order; p->fold_add adds into out (column chunks, in order).
+   cols: out[j][f] (fp32, pitch ldo) = (P^T @ F_A)[j][f] for the NBb columns of the E-step; F_A is [roundup(F,
+         SPB_TRANSFER_PANEL)][ldx] in processing order (pad rows and features zero); part: [ldx/ROW_TILE][SPB_TRANSFER_PANEL]
+         [nbb_pad] floats, by list position; the row blocks are summed in fp64 in row-block order. */
+int spb_posterior_transfer_rows(const spb_em_params* p, int32_t iter, const float* FB, int64_t ldf, int32_t F, float* part,
+                                double* out, void* stream);
+int spb_posterior_transfer_cols(const spb_em_params* p, int32_t iter, const float* FA, int32_t F, float* part, float* out,
+                                int64_t ldo, void* stream);
 
 /* ---- M-step pieces ---------------------------------------------------------------------------------------------- */
 int spb_iter_begin(const spb_em_params* p, int32_t iter, void* stream);      /* morpho_class.py:894 + zeroing */

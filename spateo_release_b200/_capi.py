@@ -135,6 +135,8 @@ def load_library():
         "spb_posterior_argmax": ([EP, I32, P, P, P], C.c_int),
         "spb_posterior_argmax_mapped": ([EP, I32, P, P, P, P], C.c_int),
         "spb_materialize_P": ([EP, I32, P, I64, P], C.c_int),
+        "spb_posterior_transfer_rows": ([EP, I32, P, I64, I32, P, P, P], C.c_int),
+        "spb_posterior_transfer_cols": ([EP, I32, P, I32, P, P, I64, P], C.c_int),
         "spb_iter_begin": ([EP, I32, P], C.c_int),
         "spb_update_gamma_alpha": ([EP, P], C.c_int),
         "spb_nonrigid_accumulate": ([EP, P], C.c_int),

@@ -86,7 +86,30 @@ def morpho_align_chain_sharded(
     return models, transformation
 
 
-def pair_device_bytes(n_moving: int, n_fixed: int, n_genes: int, chunk_cols: Optional[int] = None, n_sms: int = 132) -> int:
+def transfer_device_bytes(n_moving: int, n_fixed: int, transfer: tuple, width: int, n_sms: int = 132) -> int:
+    """Device memory of a posterior transfer with (F_B, F_A) features (0 = side not requested) when the E-step's column
+    buffers are ``width`` columns wide: F_B [n_fixed + 1][ldf] and the fp64 P @ F_B accumulator [ldf][ldx] (ldf = F_B
+    rounded up to the panel), the sweep-2 segment partials of one panel, F_A [roundup(F_A, panel)][ldx], the list-position
+    partials of one panel [row blocks][panel][width] and the fp32 P^T @ F_A of every column."""
+    from .. import _capi
+    from .morpho_class import Morpho_pairwise
+
+    W = _capi.CONST["SPB_TRANSFER_PANEL"]
+    ldx = -(-n_moving // _capi.ROW_TILE) * _capi.ROW_TILE
+    nrb = ldx // _capi.ROW_TILE
+    f_b, f_a = transfer
+    total = 0
+    if f_b:
+        ldf = -(-f_b // W) * W
+        total += 4 * (n_fixed + 1) * ldf + 8 * ldf * ldx + 4 * Morpho_pairwise._choose_segments(nrb, width, n_sms) * W * ldx
+    if f_a:
+        pad = -(-width // 8) * 8 + 8
+        total += 4 * (-(-f_a // W) * W) * ldx + 4 * nrb * W * pad + 4 * n_fixed * f_a
+    return total
+
+
+def pair_device_bytes(n_moving: int, n_fixed: int, n_genes: int, chunk_cols: Optional[int] = None, n_sms: int = 132,
+                      transfer: Optional[tuple] = None, cols: Optional[int] = None) -> int:
     """Device memory one prepared pair needs, dominated by its fp32 cost matrix [n_fixed][roundup(n_moving, 512)]; the
     expression operands of the cost precompute (two sides, value + tf32 hi / lo, genes padded to 32) and 1 GiB for the
     per-cell state are added on top.
@@ -94,12 +117,18 @@ def pair_device_bytes(n_moving: int, n_fixed: int, n_genes: int, chunk_cols: Opt
     ``chunk_cols``: the footprint of a streamed pair instead, whose cost matrix is recomputed every iteration in chunks of
     that many columns. The resident matrix is replaced by one [chunk_cols][ldx] cost chunk and every per-column buffer of
     the E-step at that width: column partials, keep masks, work lists, quarter masks, column records, the row partials
-    of the sweep's column segments (``n_sms`` sets their count) and the gathered fixed-side operands of an SVI chunk."""
+    of the sweep's column segments (``n_sms`` sets their count) and the gathered fixed-side operands of an SVI chunk.
+
+    ``transfer``: (F_B, F_A) feature counts of a posterior transfer, whose buffers (``transfer_device_bytes``) are added at
+    the chunk width, or at ``cols`` (the columns of one E-step, default ``n_fixed``) for a resident pair."""
     from .. import _capi
 
     ldx = -(-n_moving // _capi.ROW_TILE) * _capi.ROW_TILE
     gp = -(-n_genes // 32) * 32
     operands = 4 * 3 * (n_moving + n_fixed) * gp + (1 << 30)
+    if transfer is not None:
+        width = chunk_cols if chunk_cols is not None else (n_fixed if cols is None else cols)
+        operands += transfer_device_bytes(n_moving, n_fixed, transfer, width, n_sms)
     if chunk_cols is None:
         return 4 * n_fixed * ldx + operands
     from .morpho_class import Morpho_pairwise
@@ -272,8 +301,12 @@ def morpho_align_pair_sharded(fixed, moving, mode: str = "auto", device=None, **
     ``guidance_pair``, ``sparse_calculation_mode`` with ``materialize_P=True`` (one ``scipy.sparse.coo_matrix``, gathered
     from the ranks' columns, on every rank) and ``compute_mapping``. ``K_NB``, ``P`` and ``mapping`` come back in the
     unsharded column order. A dense ``materialize_P=True`` raises NotImplementedError, as does a pair whose block of the
-    cost matrix does not fit its GPU."""
+    cost matrix does not fit its GPU. ``transfer_B`` / ``transfer_A`` take keys only, as in ``morpho_align``; after
+    ``run()`` every rank holds the whole ``P_FB`` and ``PT_FA``."""
+    from .morpho_alignment import _transfer_keys
     from .morpho_class import Morpho_pairwise
+
+    _transfer_keys(pairwise_kwargs)
 
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0

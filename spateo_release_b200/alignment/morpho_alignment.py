@@ -75,6 +75,47 @@ def _store_pair(target, solver, key_added, mode, iter_key_added, vecfld_key_adde
         target.uns[vecfld_key_added] = solver.vecfld
 
 
+def _transfer_keys(kwargs) -> tuple:
+    """The posterior-transfer keywords of a driver, (transfer_B, transfer_A): keys of the slices only, since an array would
+    be ambiguous across the pairs of a chain."""
+    keys = []
+    for name in ("transfer_B", "transfer_A"):
+        v = kwargs.get(name)
+        if v is not None and not isinstance(v, str):
+            raise ValueError(f"{name}: the drivers take the name of an .obsm matrix or .obs column of the slices; an array "
+                             "is ambiguous across the pairs of a chain (pass arrays to Morpho_pairwise)")
+        keys.append(v)
+    return tuple(keys)
+
+
+def _normalise_rows(x: np.ndarray, mass: np.ndarray) -> np.ndarray:
+    """x / mass row by row (float64), rows of zero mass set to 0; float32 like the solver's outputs."""
+    x, mass = np.asarray(x, dtype=np.float64), np.asarray(mass, dtype=np.float64).reshape(-1)
+    out = np.zeros_like(x)
+    ok = mass > 0
+    out[ok] = x[ok] / mass[ok, None]
+    return out.astype(np.float32)
+
+
+def _store_transfer(fixed, moving, solver, key_B: Optional[str], key_A: Optional[str]):
+    """Posterior-weighted features of one pair: ``moving.obsm[f"{key_B}_from_fixed"] = P_FB / K_NA`` and
+    ``fixed.obsm[f"{key_A}_from_moving"] = PT_FA / K_NB``; for an ``.obs`` key also ``obs[...]`` = the category of the row
+    maximum (missing for a row of zero mass)."""
+    import pandas as pd
+
+    for key, target, res, mass, cats, suffix in (
+        (key_B, moving, solver.P_FB, solver.K_NA, solver.transfer_categories["B"], "_from_fixed"),
+        (key_A, fixed, solver.PT_FA, solver.K_NB, solver.transfer_categories["A"], "_from_moving"),
+    ):
+        if key is None:
+            continue
+        norm = _normalise_rows(res, mass)
+        target.obsm[key + suffix] = norm
+        if cats is not None:
+            codes = np.where(norm.max(axis=1) > 0, norm.argmax(axis=1), -1)
+            target.obs[key + suffix] = pd.Categorical.from_codes(codes, categories=cats)
+
+
 def morpho_align(
     models: List, rep_layer: Rep = "X", rep_field: Rep = "layer", genes: Optional[Union[List[str], np.ndarray]] = None,
     spatial_key: str = "spatial", key_added: str = "align_spatial", iter_key_added: Optional[str] = "iter_spatial",
@@ -82,7 +123,13 @@ def morpho_align(
     dtype: str = "float32", device: str = "cpu", verbose: bool = True, **kwargs,
 ) -> Tuple[List, List[np.ndarray]]:
     """Serial alignment of consecutive slices; pair i+1 starts from pair i's aligned coordinates
-    (morpho_alignment.py:22-111). Returns ``(align_models, pis)`` with ``pis[i] = P.T``."""
+    (morpho_alignment.py:22-111). Returns ``(align_models, pis)`` with ``pis[i] = P.T``.
+
+    ``transfer_B`` / ``transfer_A`` (keys only): for every pair, the fixed slice's ``.obsm`` matrix / ``.obs`` column
+    ``transfer_B`` carried to the moving slice through the pair's posterior, ``moving.obsm[f"{key}_from_fixed"] = P_FB /
+    K_NA``, and the moving slice's ``transfer_A`` to the fixed one, ``fixed.obsm[f"{key}_from_moving"] = PT_FA / K_NB`` (rows
+    of zero mass 0; an ``.obs`` key also gets ``obs[...]``, the category of the row maximum)."""
+    transfer_keys = _transfer_keys(kwargs)
     aligned = [_working_copy(m) for m in models]
     _seed_keys(aligned, spatial_key, key_added)
     # the posterior of a pair whose cost matrix is streamed (too large for the device) is not built: its entry of pis is None
@@ -95,6 +142,7 @@ def morpho_align(
             max_iter=max_iter, dtype=dtype, device=device, verbose=verbose, **kwargs,
         )
         _store_pair(moving, solver, key_added, mode, iter_key_added, vecfld_key_added)
+        _store_transfer(fixed, moving, solver, *transfer_keys)
         pis.append(None if P is None else P.T)
         del solver
         empty_cache(device=device)

@@ -144,18 +144,19 @@ class CostPlan(NamedTuple):
         return len(self.chunks)
 
 
-def plan_cost(n_moving: int, n_fixed: int, n_genes: int, cols: int, budget: int, n_sms: int = 132) -> CostPlan:
+def plan_cost(n_moving: int, n_fixed: int, n_genes: int, cols: int, budget: int, n_sms: int = 132,
+              transfer: Optional[tuple] = None) -> CostPlan:
     """Resident when ``pair_device_bytes`` fits ``budget``; otherwise the widest multiple of 8 columns (at most ``cols``,
     the columns of one iteration) whose streamed footprint fits, balanced over the chunks it takes. Raises MemoryError
-    when not even 8 columns fit."""
+    when not even 8 columns fit. ``transfer``: the feature counts (F_B, F_A) of a posterior transfer (``pair_device_bytes``)."""
     from .distributed import pair_device_bytes
 
-    need = pair_device_bytes(n_moving, n_fixed, n_genes)
+    need = pair_device_bytes(n_moving, n_fixed, n_genes, transfer=transfer, n_sms=n_sms, cols=cols)
     if need <= budget:
         return CostPlan("resident", cols, ((0, cols),), need, budget)
 
     def need_at(c):
-        return pair_device_bytes(n_moving, n_fixed, n_genes, chunk_cols=c, n_sms=n_sms)
+        return pair_device_bytes(n_moving, n_fixed, n_genes, chunk_cols=c, n_sms=n_sms, transfer=transfer)
 
     if need_at(min(8, cols)) > budget:
         raise MemoryError(
@@ -176,6 +177,43 @@ def plan_cost(n_moving: int, n_fixed: int, n_genes: int, cols: int, budget: int,
     width = min(cols, _round_up(-(-cols // n), 8))  # same chunk count, widths as even as multiples of 8 allow
     chunks = tuple((c0, min(cols, c0 + width)) for c0 in range(0, cols, width))
     return CostPlan("streamed", width, chunks, need_at(width), budget)
+
+
+def resolve_transfer(adata, spec, n_rows: int, name: str):
+    """Features of a posterior transfer on one slice: ``spec`` is a float array [n_rows, F] in the slice's row order, the
+    name of an ``.obsm`` matrix, or the name of an ``.obs`` column, one-hot encoded in ``pd.Categorical(...).categories``
+    order (a missing value is an all-zero row). Returns (float32 [n_rows, F], categories or None); ``ValueError`` for a
+    missing key, a row count other than ``n_rows``, F = 0 or a non-finite value."""
+    import pandas as pd
+
+    cats = None
+    if isinstance(spec, str):
+        if spec in adata.obsm:
+            arr = adata.obsm[spec]
+            arr = arr.values if isinstance(arr, pd.DataFrame) else (arr.toarray() if hasattr(arr, "toarray") else arr)
+        elif spec in adata.obs.columns:
+            cat = pd.Categorical(adata.obs[spec])
+            cats = list(cat.categories)
+            codes = np.asarray(cat.codes)
+            arr = np.zeros((codes.shape[0], len(cats)), dtype=np.float32)
+            arr[np.flatnonzero(codes >= 0), codes[codes >= 0]] = 1.0
+        else:
+            raise ValueError(f"{name}: '{spec}' is neither an .obsm matrix nor an .obs column of the slice")
+    else:
+        arr = spec
+    try:
+        arr = np.asarray(arr, dtype=np.float64)
+    except (TypeError, ValueError) as e:
+        raise ValueError(f"{name}: the features must be numeric ({e})") from None
+    if arr.ndim != 2:
+        raise ValueError(f"{name}: expected a [cells, features] matrix, got shape {arr.shape}")
+    if arr.shape[0] != n_rows:
+        raise ValueError(f"{name}: {arr.shape[0]} rows for a slice of {n_rows} cells")
+    if arr.shape[1] == 0:
+        raise ValueError(f"{name}: no features (F = 0)")
+    if not np.isfinite(arr).all():
+        raise ValueError(f"{name}: the features hold non-finite values")
+    return arr.astype(np.float32), cats
 
 
 def svi_schedule(batch_perm: np.ndarray, max_iter: int, nbb: int) -> np.ndarray:
@@ -354,6 +392,13 @@ class Morpho_pairwise:
     ``kernel_type="geodist"``, any K, ``sparse_calculation_mode``, ``return_mapping`` and ``iter_key_added``; it refuses
     (NotImplementedError) dense ``materialize_P=True``, ``compute_mapping`` and ``column_shard``. With one chunk (default SVI)
     its results are bit-identical to the resident run.
+    ``transfer_B`` / ``transfer_A`` — carry cell features through the final posterior without forming it: ``P_FB = P @
+    F_B`` ([N_A, F], the caller's row order of ``sampleA``) and ``PT_FA = P^T @ F_A`` ([n_cols, F], P's column order, that
+    of ``K_NB``), un-normalised float32, ``None`` when not requested. Each is a float array in the slice's row order
+    ([N_B, F] for ``transfer_B``, [N_A, F] for ``transfer_A``), an ``.obsm`` key, or an ``.obs`` key one-hot encoded in
+    category order (``transfer_categories = {"A": [...], "B": [...]}``). The posterior is the one ``run()`` returns as P:
+    that of the last E-step (sparse mode: the kept entries w >= tau_j). Under ``SVI_mode`` a transfer requires
+    ``return_mapping=True``, whose closing E-step covers every fixed cell. Resident, streamed and column-sharded pairs.
     Accepted but without effect (memory work-arounds whose results are identical): ``use_chunk``, ``chunk_capacity``,
     ``pre_compute_dist``. ``sparse_calculation_mode`` keeps the top ``sparse_top_k`` posterior entries of every column by an
     exact on-device radix select (P comes back as ``scipy.sparse.coo_matrix``). Not implemented (NotImplementedError):
@@ -422,6 +467,8 @@ class Morpho_pairwise:
         spatial_sort: bool = True,
         cull_zero_tiles: bool = True,
         column_shard=None,
+        transfer_B=None,
+        transfer_A=None,
     ) -> None:
         self.verbose = verbose
         self.sampleA, self.sampleB = sampleA, sampleB
@@ -463,6 +510,7 @@ class Morpho_pairwise:
 
         self._np_dtype = np.float32 if dtype == "float32" else np.float64
         self._check()
+        self._check_transfer(transfer_B, transfer_A)
         self._lib = _capi.load_library()
         self._dev = resolve_device(device)
         with torch.cuda.device(self._dev):
@@ -546,6 +594,32 @@ class Morpho_pairwise:
                 f"dtype={self.dtype!r} is not implemented in spateo_release_b200: the device path computes in float32 "
                 "(fp64 reductions / solves); use dtype='float32'."
             )
+
+    def _check_transfer(self, transfer_B, transfer_A):
+        """Posterior-transfer features of both slices (``resolve_transfer``); under SVI only with ``return_mapping``."""
+        self.P_FB = self.PT_FA = None
+        self.transfer_categories = {"A": None, "B": None}
+        self._FB_host = self._FA_host = None
+        if transfer_B is None and transfer_A is None:
+            return
+        if self.SVI_mode and not self.return_mapping:
+            raise ValueError("transfer_B / transfer_A under SVI_mode=True need return_mapping=True: the last SVI posterior "
+                             "covers one batch of fixed cells, the closing E-step of return_mapping covers all of them")
+        nA, nB = self.sampleA.obsm[self.spatial_key].shape[0], self.sampleB.obsm[self.spatial_key].shape[0]
+        if transfer_B is not None:
+            self._FB_host, self.transfer_categories["B"] = resolve_transfer(self.sampleB, transfer_B, nB, "transfer_B")
+        if transfer_A is not None:
+            self._FA_host, self.transfer_categories["A"] = resolve_transfer(self.sampleA, transfer_A, nA, "transfer_A")
+
+    @property
+    def _transfer_on(self) -> bool:
+        return self._FB_host is not None or self._FA_host is not None
+
+    def _transfer_dims(self) -> Optional[tuple]:
+        """Feature counts (F_B, F_A) of the requested transfer (0 = that side not requested), None without one."""
+        if not self._transfer_on:
+            return None
+        return tuple(0 if f is None else f.shape[1] for f in (self._FB_host, self._FA_host))
 
     # ------------------------------------------------------------------------------------------------------------------
     # preprocessing (morpho_class.py:443-558)
@@ -977,7 +1051,8 @@ class Morpho_pairwise:
         """Resident or streamed cost matrix, from the pair's size and the memory the device has (``plan_cost``)."""
         cols = min(self.batch_size, nb_loc) if self.SVI_mode else nb_loc
         n_sms = torch.cuda.get_device_properties(self._dev).multi_processor_count
-        plan = plan_cost(self.NA, nb_loc, self._cost_features(), cols, _device_budget(self._dev), n_sms)
+        plan = plan_cost(self.NA, nb_loc, self._cost_features(), cols, _device_budget(self._dev), n_sms,
+                         transfer=self._transfer_dims())
         if isinstance(self.materialize_P, str) and self.materialize_P == "auto":  # the public drivers' default
             self.materialize_P = not plan.streamed
         if plan.streamed:
@@ -1334,6 +1409,67 @@ class Morpho_pairwise:
             p.UT_hi = p.UT_lo = p.UT_mean = p.GB_hi = p.GB_lo = p.gram_scratch = p.gram_sums = None
             p.gram_scratch_floats = 0
         self._params = p
+        if self._transfer_on:
+            self._allocate_transfer(s, NB, nrb)
+
+    def _allocate_transfer(self, s, nb_loc: int, nrb: int):
+        """Device buffers of the posterior transfer: F_B [nb_loc + 1][ldf] (this process's fixed cells, then the zero row of
+        an SVI shard's null column; ldf = F rounded up to the panel width, so every panel row is 64-byte aligned), F_A
+        [roundup(F, panel)][ldx] in processing order, the fp64 P @ F_B accumulator [ldf][ldx], and the partials of the two
+        kernels: [segments][panel][ldx] (P @ F_B) and [row blocks][panel][nbb_pad] by list position (P^T @ F_A)."""
+        W, dev, ldx, f32 = _capi.CONST["SPB_TRANSFER_PANEL"], self._dev, self.ldx, torch.float32
+        if self._FB_host is not None:
+            c0, c1 = self._col_range()
+            F = self._FB_host.shape[1]
+            fb = torch.zeros((nb_loc + 1, _round_up(F, W)), dtype=f32, device=dev)
+            fb[:nb_loc, :F] = torch.from_numpy(self._FB_host[c0:c1]).to(dev)
+            s["xfer_FB"] = fb
+            s["xfer_PFB"] = torch.zeros((fb.shape[1], ldx), dtype=torch.float64, device=dev)
+            s["xfer_rowpart"] = torch.zeros((s["rowpart"].shape[0], W, ldx), dtype=f32, device=dev)
+        if self._FA_host is not None:
+            F = self._FA_host.shape[1]
+            fa = torch.zeros((_round_up(F, W), ldx), dtype=f32, device=dev)
+            fa[:F, : self.NA] = torch.from_numpy(np.ascontiguousarray(self._sorted(self._FA_host).T)).to(dev)
+            s["xfer_FA"] = fa
+            s["xfer_colpart"] = torch.zeros((nrb, W, self._nbb_pad), dtype=f32, device=dev)
+
+    def _transfer_begin(self):
+        """Output of P^T @ F_A for the columns of the E-step about to be captured (P @ F_B accumulates in xfer_PFB)."""
+        if self._FA_host is not None:
+            self._xfer_PTFA = torch.zeros((self._NBb, self._FA_host.shape[1]), dtype=torch.float32, device=self._dev)
+
+    def _transfer_capture(self, q: SpbEmParams, it: int, st, c0: int = 0):
+        """P @ F_B and P^T @ F_A of the E-step that ``q`` describes, while its lists and column constants are live: the
+        whole E-step, or its column chunk [c0, c0 + q.NBb) (P @ F_B is added in chunk order through ``q.fold_add``)."""
+        lib, s = self._lib, self._state
+        if self._FB_host is not None:
+            fb = s["xfer_FB"]
+            # the F_B rows follow xb4: a full-EM chunk's columns are fixed cells c0.., an SVI chunk's schedule is global
+            base = fb.data_ptr() + (0 if q.svi else c0) * fb.shape[1] * 4
+            check(lib.spb_posterior_transfer_rows(C.byref(q), it, C.c_void_p(base), fb.shape[1], self._FB_host.shape[1],
+                                                  ptr(s["xfer_rowpart"]), ptr(s["xfer_PFB"]), st),
+                  "spb_posterior_transfer_rows")
+        if self._FA_host is not None:
+            F = self._FA_host.shape[1]
+            out = self._xfer_PTFA[c0:]
+            check(lib.spb_posterior_transfer_cols(C.byref(q), it, ptr(s["xfer_FA"]), F, ptr(s["xfer_colpart"]), ptr(out), F,
+                                                  st), "spb_posterior_transfer_cols")
+
+    def _transfer_results(self, n_cols: int):
+        """``P_FB`` (caller's row order) and ``PT_FA`` (P's column order) of the captured posterior, float32 like the other
+        outputs. A column-sharded pair sums the ranks' P @ F_B in fp64 in rank order and gathers P^T @ F_A by column."""
+        s = self._state
+        if self._FB_host is not None:
+            acc = s["xfer_PFB"]
+            if self.column_shard is not None:
+                self._shard_sum_tensor(acc)
+            pfb = acc[: self._FB_host.shape[1], : self.NA].T.contiguous().to(torch.float32)
+            _count_d2h(pfb)
+            self.P_FB = self._unsorted(pfb.cpu().numpy())
+        if self._FA_host is not None:
+            t = self._xfer_PTFA
+            self.PT_FA = self._shard_columns(t, n_cols) if self.column_shard is not None else t.cpu().numpy()
+            self._xfer_PTFA = None
 
     def _setup_column_shard(self, p, s):
         """Buffers of the column-sharded pair: fp64 row statistics of this rank's columns (double-buffered) + epoch flags.
@@ -1400,6 +1536,18 @@ class Morpho_pairwise:
 
             if dist.is_initialized() and dist.get_world_size() > 1:
                 dist.all_reduce(view)
+
+    def _shard_sum_tensor(self, t: torch.Tensor):
+        """In place: the sum of every rank's fp64 ``t`` through the collective, whatever the row-statistics mode (the
+        peer-memory kernel sums only those)."""
+        comm = getattr(self, "_shard_comm", None)
+        if comm is not None:
+            comm.sum_(self, t)
+        else:
+            import torch.distributed as dist
+
+            if dist.is_initialized() and dist.get_world_size() > 1:
+                dist.all_reduce(t)
 
     def _shard_finish_rows(self, st):
         """Finish the row statistics from the view of ``_shard_fold`` once ``_shard_sum`` made it the sum over the ranks
@@ -1573,6 +1721,9 @@ class Morpho_pairwise:
         """Posterior of the E-step that has just run: dense [N_A, NBb], or in sparse_calculation_mode the COO entries
         (top-k rows and values per column) without ever forming the dense matrix."""
         lib, p = self._lib, self._params
+        if self._transfer_on:
+            self._transfer_begin()
+            self._transfer_capture(p, it, st)
         if self.compute_mapping:  # row / column maxima of the same posterior, straight from the cost matrix
             self._rowbest = torch.zeros((self.NA,), dtype=torch.int64, device=self._dev)
             self._colbest = torch.zeros((self._NBb,), dtype=torch.int64, device=self._dev)
@@ -1691,21 +1842,33 @@ class Morpho_pairwise:
         check(lib.spb_row_stats_finalize(C.byref(p), 0, st), "spb_row_stats_finalize")
 
     def _streamed_capture(self):
-        """Posterior capture of a streamed E-step (sparse mode only: the COO entries of every chunk's columns, emitted while
-        the chunk is live); None when nothing is captured."""
-        if not (self.materialize_P and self.sparse_calculation_mode):
+        """Posterior capture of a streamed E-step, run on every chunk while it is live: the COO entries of its columns
+        (sparse mode) and the posterior transfer; None when nothing is captured."""
+        hooks = []
+        if self.materialize_P and self.sparse_calculation_mode:
+            k = int(self.sparse_top_k)
+            self._P_rows = torch.zeros((self._NBb, k), dtype=torch.int32, device=self._dev)
+            self._P_vals = torch.zeros((self._NBb, k), dtype=torch.float32, device=self._dev)
+            self._P_dev = "sparse"
+
+            def emit(q, it, c0, c1):
+                check(self._lib.spb_sparse_P_emit(C.byref(q), it, ptr(self._P_rows[c0:c1]), ptr(self._P_vals[c0:c1]),
+                                                  _capi.current_stream_ptr()), "spb_sparse_P_emit")
+
+            hooks.append(emit)
+        else:
             self._P_dev = "skipped"
+        if self._transfer_on:
+            self._transfer_begin()
+            hooks.append(lambda q, it, c0, c1: self._transfer_capture(q, it, _capi.current_stream_ptr(), c0))
+        if not hooks:
             return None
-        k = int(self.sparse_top_k)
-        self._P_rows = torch.zeros((self._NBb, k), dtype=torch.int32, device=self._dev)
-        self._P_vals = torch.zeros((self._NBb, k), dtype=torch.float32, device=self._dev)
-        self._P_dev = "sparse"
 
-        def emit(q, it, c0, c1):
-            check(self._lib.spb_sparse_P_emit(C.byref(q), it, ptr(self._P_rows[c0:c1]), ptr(self._P_vals[c0:c1]),
-                                              _capi.current_stream_ptr()), "spb_sparse_P_emit")
+        def capture(q, it, c0, c1):
+            for h in hooks:
+                h(q, it, c0, c1)
 
-        return emit
+        return capture
 
     def prepare_host(self):
         """Coarse rigid initialisation + variational initialisation (host numpy with small device helpers); consumes
@@ -1765,14 +1928,14 @@ class Morpho_pairwise:
             it, end = start, start + n_iter
             while it < end:
                 last = it == self.max_iter - 1
-                want_P = (self.materialize_P or self.compute_mapping) and last and not (self.return_mapping and self.SVI_mode)
+                want_P = self._captures_posterior and last and not (self.return_mapping and self.SVI_mode)
                 nonrigid = it > self.nonrigid_start_iter
                 plain = (hist is not None or sweep_events is not None or want_P or self.column_shard is not None
                          or self._streamed or (nonrigid and self.K > _capi.MAX_K_FUSED))
                 if not plain:
                     # iterations [it, stop) share the phase and need nothing from the host
                     stop = min(end, self.nonrigid_start_iter + 1) if not nonrigid else end
-                    if (self.materialize_P or self.compute_mapping) and stop == self.max_iter and not (self.return_mapping and self.SVI_mode):
+                    if self._captures_posterior and stop == self.max_iter and not (self.return_mapping and self.SVI_mode):
                         stop -= 1  # the last iteration captures the posterior: plain path
                     if stop - it >= 3:
                         self._iteration(it, st)  # explicit index: also the warm-up launch of every kernel of the phase
@@ -1804,6 +1967,11 @@ class Morpho_pairwise:
                     self._state["hist_sigma2"][it].copy_(self._state["sc"][:8].view(torch.float64)[0])
                 self._iteration(it, st, capture_P=want_P, sweep_events=sweep_events)
                 it += 1
+
+    @property
+    def _captures_posterior(self) -> bool:
+        """The posterior of the final E-step has a consumer: dense / sparse P, the mapping or the transfer."""
+        return bool(self.materialize_P or self.compute_mapping or self._transfer_on)
 
     def _graph_unroll(self) -> int:
         """Iterations per captured graph: 8 when an iteration touches fewer than 2e9 cell pairs (about 2 ms of device time:
@@ -1925,8 +2093,10 @@ class Morpho_pairwise:
         else:
             self.Coff = np.zeros(self.K, dtype=dt)  # the reference's initial value (morpho_class.py:733)
         self.trace = s["trace_buf"].cpu().numpy()
-        if (self.materialize_P or self.compute_mapping) and getattr(self, "_P_dev", None) is None:
+        if self._captures_posterior and getattr(self, "_P_dev", None) is None:
             self._capture_P(last_iter, st)  # max_iter == 0 or the return_mapping E-step above
+        if self._transfer_on:
+            self._transfer_results(n_cols)
         if self.compute_mapping:
             from .mapping import ArgmaxPi
 

@@ -66,11 +66,15 @@ __device__ __forceinline__ ColRange col_range(const int32_t* __restrict__ colcou
 // reads. Slots past the end of the slice have no live quarter and take the all-zero constant entry at index NBb (the
 // constant arrays are zero-padded). The stage's masks, with the spatially live quarters (colspatial) in the high nibble
 // of each byte, go to sm.quarters before the arrive on the full barrier, which publishes them with the copies.
+// kFeat > 0 (posterior transfer): a column with a live quarter also brings its kFeat-float feature panel row
+// fsrc[frow * ldf ..] (frow = fcol_index[j], or j) to fdst[stage][slot][0 .. kFeat).
+template <int kFeat = 0>
 __device__ __forceinline__ void producer_loop(SmemLayout& sm, const float* __restrict__ GT, int64_t ldx,
                                               const int32_t* __restrict__ col_index, const int32_t* __restrict__ list,
                                               const uint8_t* __restrict__ quarters, const uint8_t* __restrict__ spatial,
                                               const float* __restrict__ colsrc, int col_floats, int i0, ColRange cr, int NBb,
-                                              int lane) {
+                                              int lane, const float* __restrict__ fsrc = nullptr, int64_t ldf = 0,
+                                              const int32_t* __restrict__ fcol_index = nullptr, float* fdst = nullptr) {
   const int nst = (cr.end - cr.begin + kColStage - 1) / kColStage;
   for (int st = 0; st < nst; ++st) {
     const int s = st % kStages;
@@ -79,7 +83,7 @@ __device__ __forceinline__ void producer_loop(SmemLayout& sm, const float* __res
     const bool slot = lane < kColStage, live = slot && pb + lane < cr.end;
     const uint32_t qm = live ? quarters[pb + lane] : 0u;
     const uint32_t wm = live ? qm | (uint32_t)spatial[pb + lane] << 4 : 0u;
-    const uint32_t bytes = slot ? __popc(qm) * kQuarter * 4 + col_floats * 4 : 0u;
+    const uint32_t bytes = slot ? __popc(qm) * kQuarter * 4 + col_floats * 4 + (qm != 0u ? kFeat * 4 : 0) : 0u;
     const uint32_t total = __reduce_add_sync(0xffffffffu, bytes);
     const uint32_t lo = __reduce_or_sync(0xffffffffu, lane < 4 ? wm << (8 * lane) : 0u);
     const uint32_t hi = __reduce_or_sync(0xffffffffu, (lane >= 4 && slot) ? wm << (8 * (lane - 4)) : 0u);
@@ -98,6 +102,10 @@ __device__ __forceinline__ void producer_loop(SmemLayout& sm, const float* __res
           const int len = __ffs(~(m >> q0)) - 1;  // length of the run of set bits starting at q0
           bulk_g2s(&sm.tile[s][lane][q0 * kQuarter], src + q0 * kQuarter, len * kQuarter * 4, &sm.full[s]);
           m &= ~(((1u << len) - 1u) << q0);
+        }
+        if constexpr (kFeat > 0) {
+          const int64_t frow = fcol_index ? (int64_t)fcol_index[j] : (int64_t)j;
+          bulk_g2s(fdst + (s * kColStage + lane) * kFeat, fsrc + frow * ldf, kFeat * 4, &sm.full[s]);
         }
       }
       bulk_g2s(&sm.cols[s][lane][0], colsrc + (int64_t)j * col_floats, col_floats * 4, &sm.full[s]);
@@ -1279,6 +1287,277 @@ row_argmax_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __re
   if (j0 < j1) atomicMax(rowbest + i, best);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// posterior transfer: P @ F_B and P^T @ F_A of the last E-step without forming P
+// ---------------------------------------------------------------------------------------------------------------------
+// Both kernels visit the (row block, column) tiles and 128-row quarters of the E-step's work lists with the grid and
+// pipeline of the sweeps, and form P_ij = (q_ij g_ij) c_j with sweep 2's instruction sequence (sparse mode: w < tau_j
+// is absent). Features are processed in panels of kXferPanel; a panel reads the listed cost tiles once. Skipped pairs
+// are exact zeros, so culling changes no bit. No float atomics: every fold has a fixed order.
+constexpr int kXferPanel = SPB_TRANSFER_PANEL;
+constexpr int kXferCtas = 3;  // 4 x 16 fp32 accumulators (or feature registers) per thread: 3 CTAs of 160 threads per SM
+static_assert(kXferPanel == 16, "one butterfly of 16 values per column, two 32-byte sectors per feature and stage");
+
+struct __align__(16) XferSmem {
+  SmemLayout base;
+  float fpan[kStages][kColStage][kXferPanel];           // rows kernel: F_B panel rows of the staged columns
+  float red[2][kColStage][kConsumers / 32][kXferPanel];  // cols kernel: warp totals of the staged columns
+};
+
+// P of this thread's 4 rows with staged column jj (a column whose q bit is set for the warp)
+template <bool kSparse, int kDim>
+__device__ __forceinline__ void xfer_weights(const SmemLayout& sm, int s, int jj, int tid, const RowRegs& R, u64 CQ,
+                                             float (&p)[4]) {
+  const ulonglong2 c0 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][0]);  // (y0,y0) (y1,y1)
+  const ulonglong2 c1 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][1]);  // (y2,y2) (a,a)
+  const ulonglong2 c2 = *reinterpret_cast<const ulonglong2*>(&sm.cols[s][jj][2]);  // (b,b)  (c,c)
+  const ulonglong2 g = *reinterpret_cast<const ulonglong2*>(&sm.tile[s][jj][tid * 4]);
+  const u64 da = sqdist2<kDim>(R.xa0, R.xa1, R.xa2, c0.x, c0.y, c1.x);
+  const u64 db = sqdist2<kDim>(R.xb0, R.xb1, R.xb2, c0.x, c0.y, c1.x);
+  const u64 qa = ex2_2(fma2(CQ, da, R.lma)), qb = ex2_2(fma2(CQ, db, R.lmb));
+  u64 wa = mul2(qa, g.x), wb = mul2(qb, g.y);
+  if constexpr (kSparse) {
+    const float tau = sm.cols[s][jj][4].z;
+    wa = keep_ge(wa, tau);
+    wb = keep_ge(wb, tau);
+  }
+  upk(mul2(wa, c2.y), p[0], p[1]);
+  upk(mul2(wb, c2.y), p[2], p[3]);
+}
+
+// P @ F_B, one feature panel: grid and pipeline of sweep 2; per-segment fp32 partials part[seg][kXferPanel][ldx]
+template <bool kSparse, int kDim = 3>
+__global__ void __launch_bounds__(kThreads, kXferCtas)
+transfer_rows_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __restrict__ batch_base,
+                     const int32_t* __restrict__ fbatch_base, const float* __restrict__ colconst,
+                     const float* __restrict__ XA, const float* __restrict__ lm, const spb_scalars* __restrict__ sc,
+                     const float* __restrict__ FB, int64_t ldf, float* __restrict__ part, int NBb, int nbb_pad,
+                     const int32_t* __restrict__ collist, const uint8_t* __restrict__ colquarters,
+                     const uint8_t* __restrict__ colspatial, const int32_t* __restrict__ colcount) {
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  XferSmem& xs = *reinterpret_cast<XferSmem*>(smem_raw);
+  SmemLayout& sm = xs.base;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int rb = blockIdx.x, seg = blockIdx.y;
+  const int i0 = rb * kRowTile;
+  const ColRange cr = col_range(colcount, rb, seg, gridDim.y);
+  if (tid == 0) {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&sm.full[s], 1);
+      mbar_init(&sm.empty[s], kConsumers / 32);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  const int nst = cr.begin < cr.end ? (cr.end - cr.begin + kColStage - 1) / kColStage : 0;
+  if (warp == kConsumers / 32) {
+    if (nst > 0)
+      producer_loop<kXferPanel>(sm, GT, ldx, batch_cols(batch_base, sc, NBb), collist + (int64_t)rb * nbb_pad,
+                                colquarters + (int64_t)rb * nbb_pad, colspatial + (int64_t)rb * nbb_pad, colconst,
+                                SPB_COLCONST_FLOATS, i0, cr, NBb, lane, FB, ldf, batch_cols(fbatch_base, sc, NBb),
+                                &xs.fpan[0][0][0]);
+    return;
+  }
+  const u64 CQ = pk(sc->c_q, sc->c_q);
+  const int r = i0 + tid * 4;
+  const RowRegs R = load_rows(XA, ldx, lm, nullptr, r);
+  float acc[4][kXferPanel];
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+#pragma unroll
+    for (int f = 0; f < kXferPanel; ++f) acc[q][f] = 0.f;
+  for (int st = 0; st < nst; ++st) {
+    const int s = st % kStages;
+    mbar_wait(&sm.full[s], (st / kStages) & 1);
+    const uint64_t wq = sm.quarters[s] >> warp;
+#pragma unroll
+    for (int jj = 0; jj < kColStage; ++jj) {
+      if (!quarter_q(wq, jj)) continue;
+      float p[4];
+      xfer_weights<kSparse, kDim>(sm, s, jj, tid, R, CQ, p);
+      const float4* fr = reinterpret_cast<const float4*>(&xs.fpan[s][jj][0]);
+#pragma unroll
+      for (int v = 0; v < kXferPanel / 4; ++v) {
+        const float4 f = fr[v];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          acc[q][4 * v + 0] = fmaf(p[q], f.x, acc[q][4 * v + 0]);
+          acc[q][4 * v + 1] = fmaf(p[q], f.y, acc[q][4 * v + 1]);
+          acc[q][4 * v + 2] = fmaf(p[q], f.z, acc[q][4 * v + 2]);
+          acc[q][4 * v + 3] = fmaf(p[q], f.w, acc[q][4 * v + 3]);
+        }
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&sm.empty[s]);
+  }
+  float* out = part + (int64_t)seg * kXferPanel * ldx + r;
+#pragma unroll
+  for (int f = 0; f < kXferPanel; ++f)
+    *reinterpret_cast<float4*>(out + (int64_t)f * ldx) = make_float4(acc[0][f], acc[1][f], acc[2][f], acc[3][f]);
+}
+
+// per moving cell: the segment partials of one panel folded in fp64 in segment order (row_finalize), written to or (add:
+// the next column chunk of a streamed E-step) added into out[kXferPanel][ldx]
+__global__ void __launch_bounds__(256)
+transfer_row_fold_kernel(const float* __restrict__ part, int nseg, int ldx, int NA, int add, double* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= NA) return;
+#pragma unroll 4
+  for (int f = 0; f < kXferPanel; ++f) {
+    double a = 0.0;
+    for (int s = 0; s < nseg; ++s) a += (double)part[((int64_t)s * kXferPanel + f) * ldx + i];
+    double* o = out + (int64_t)f * ldx + i;
+    *o = add ? *o + a : a;
+  }
+}
+
+// P^T @ F_A, one feature panel: grid and pipeline of sweep 1. Each consumer thread holds its 4 rows of the panel; per
+// staged column a warp reduces its quarter with the butterfly, warp 0 adds the four warps in order (sweep 1) and stores
+// the row block's partials by list position, part[rb][kXferPanel][nbb_pad]: one 32-byte sector per feature and stage.
+template <bool kSparse, int kDim = 3>
+__global__ void __launch_bounds__(kThreads, kXferCtas)
+transfer_cols_kernel(const float* __restrict__ GT, int64_t ldx, const int32_t* __restrict__ batch_base,
+                     const float* __restrict__ colconst, const float* __restrict__ XA, const float* __restrict__ lm,
+                     const spb_scalars* __restrict__ sc, const float* __restrict__ FA, float* __restrict__ part, int NBb,
+                     int nbb_pad, const int32_t* __restrict__ collist, const uint8_t* __restrict__ colquarters,
+                     const uint8_t* __restrict__ colspatial, const int32_t* __restrict__ colcount) {
+  extern __shared__ __align__(128) uint8_t smem_raw[];
+  XferSmem& xs = *reinterpret_cast<XferSmem*>(smem_raw);
+  SmemLayout& sm = xs.base;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int rb = blockIdx.x, seg = blockIdx.y;
+  const int i0 = rb * kRowTile;
+  const ColRange cr = col_range(colcount, rb, seg, gridDim.y);
+  if (cr.begin >= cr.end) return;
+  if (tid == 0) {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&sm.full[s], 1);
+      mbar_init(&sm.empty[s], kConsumers / 32);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (warp == kConsumers / 32) {
+    producer_loop(sm, GT, ldx, batch_cols(batch_base, sc, NBb), collist + (int64_t)rb * nbb_pad,
+                  colquarters + (int64_t)rb * nbb_pad, colspatial + (int64_t)rb * nbb_pad, colconst, SPB_COLCONST_FLOATS,
+                  i0, cr, NBb, lane);
+    return;
+  }
+  const u64 CQ = pk(sc->c_q, sc->c_q);
+  const int r = i0 + tid * 4;
+  const RowRegs R = load_rows(XA, ldx, lm, nullptr, r);
+  float fa[kXferPanel][4];
+#pragma unroll
+  for (int f = 0; f < kXferPanel; ++f) {
+    const float4 v = *reinterpret_cast<const float4*>(FA + (int64_t)f * ldx + r);
+    fa[f][0] = v.x, fa[f][1] = v.y, fa[f][2] = v.z, fa[f][3] = v.w;
+  }
+  float* out = part + (int64_t)rb * kXferPanel * nbb_pad;
+  const int nst = (cr.end - cr.begin + kColStage - 1) / kColStage;
+  for (int st = 0; st < nst; ++st) {
+    const int s = st % kStages;
+    mbar_wait(&sm.full[s], (st / kStages) & 1);
+    const int pb = cr.begin + st * kColStage;
+    const int buf = st & 1;
+    const uint64_t wq = sm.quarters[s] >> warp;
+#pragma unroll
+    for (int jj = 0; jj < kColStage; ++jj) {
+      float v[kXferPanel];
+      if (quarter_q(wq, jj)) {
+        float p[4];
+        xfer_weights<kSparse, kDim>(sm, s, jj, tid, R, CQ, p);
+#pragma unroll
+        for (int f = 0; f < kXferPanel; ++f)
+          v[f] = fmaf(p[3], fa[f][3], fmaf(p[2], fa[f][2], fmaf(p[1], fa[f][1], p[0] * fa[f][0])));
+      } else {
+#pragma unroll
+        for (int f = 0; f < kXferPanel; ++f) v[f] = 0.f;
+      }
+      butterfly_reduce<kXferPanel>(v, lane);  // lanes 2f and 2f + 1: the warp total of feature f
+      if ((lane & 1) == 0) xs.red[buf][jj][warp][lane >> 1] = v[0];
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&sm.empty[s]);
+    named_bar_sync(1, kConsumers);
+    if (warp == 0) {
+      const int f = lane >> 1, j0 = (lane & 1) * 4;
+      float t[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        t[k] = 0.f;
+#pragma unroll
+        for (int w = 0; w < kConsumers / 32; ++w) t[k] += xs.red[buf][j0 + k][w][f];
+      }
+      // segments begin at multiples of kColStage and only the last one of a list ends inside a stage: the positions past
+      // the list's end hold zeros that no fold reads
+      *reinterpret_cast<float4*>(out + (int64_t)f * nbb_pad + pb + j0) = make_float4(t[0], t[1], t[2], t[3]);
+    }
+  }
+}
+
+// per column: the row blocks' partials of one panel summed in fp64 in row-block order, found by list position with the
+// keepmask / livemask / keepoff lookup of col_finalize; out[j][0 .. nf) of the [NBb][ldo] result
+__global__ void __launch_bounds__(128)
+transfer_col_fold_kernel(const float* __restrict__ part, const uint32_t* __restrict__ keepmask,
+                         const uint32_t* __restrict__ livemask, const int2* __restrict__ keepoff, int kstride, int nrb,
+                         int nbb_pad, int NBb, int nf, float* __restrict__ out, int64_t ldo) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= NBb) return;
+  const int wd = j >> 5, bit = j & 31;
+  const uint32_t below = (1u << bit) - 1u;
+  double C[kXferPanel];
+#pragma unroll
+  for (int f = 0; f < kXferPanel; ++f) C[f] = 0.0;
+  for (int rb = 0; rb < nrb; ++rb) {
+    const int64_t w = (int64_t)rb * kstride + wd;
+    const uint32_t bits = keepmask[w];
+    if (((bits >> bit) & 1u) == 0u) continue;
+    const uint32_t lbits = livemask[w];
+    const int2 off = keepoff[w];
+    const int pos = ((lbits >> bit) & 1u) ? off.x + __popc(lbits & below) : off.y + __popc(bits & ~lbits & below);
+    const float* q = part + (int64_t)rb * kXferPanel * nbb_pad + pos;
+#pragma unroll
+    for (int f = 0; f < kXferPanel; ++f) C[f] += (double)q[(int64_t)f * nbb_pad];
+  }
+#pragma unroll
+  for (int f = 0; f < kXferPanel; ++f)
+    if (f < nf) out[(int64_t)j * ldo + f] = (float)C[f];
+}
+
+template <typename K>
+int xfer_smem_opt_in(K kernel, bool (&attr_set)[SPB_MAX_DEVICES]) {
+  const int dev_ = spb_current_device();
+  if (attr_set[dev_]) return 0;
+  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(XferSmem));
+  if (e != cudaSuccess) return (int)e;
+  e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e != cudaSuccess) return (int)e;
+  attr_set[dev_] = true;
+  return 0;
+}
+
+template <bool SP, int DIM>
+int launch_transfer_rows(const spb_em_params* p, const int32_t* gtb, const int32_t* fb, const float* FB, int64_t ldf,
+                         float* part, cudaStream_t st) {
+  static bool attr_set[SPB_MAX_DEVICES] = {};
+  if (int rc = xfer_smem_opt_in(transfer_rows_kernel<SP, DIM>, attr_set)) return rc;
+  transfer_rows_kernel<SP, DIM><<<dim3(p->ldx / kRowTile, p->seg2), kThreads, sizeof(XferSmem), st>>>(
+      p->GT, p->ldx, gtb, fb, p->colconst, p->XAHat, p->lm, p->sc, FB, ldf, part, p->NBb, p->nbb_pad, p->collist,
+      p->colquarters, p->colspatial, p->colcount);
+  return 0;
+}
+
+template <bool SP, int DIM>
+int launch_transfer_cols(const spb_em_params* p, const int32_t* gtb, const float* FA, float* part, cudaStream_t st) {
+  static bool attr_set[SPB_MAX_DEVICES] = {};
+  if (int rc = xfer_smem_opt_in(transfer_cols_kernel<SP, DIM>, attr_set)) return rc;
+  transfer_cols_kernel<SP, DIM><<<dim3(p->ldx / kRowTile, p->seg1), kThreads, sizeof(XferSmem), st>>>(
+      p->GT, p->ldx, gtb, p->colconst, p->XAHat, p->lm, p->sc, FA, part, p->NBb, p->nbb_pad, p->collist, p->colquarters,
+      p->colspatial, p->colcount);
+  return 0;
+}
+
 template <int DIM = 3>
 int launch_sweep1(const spb_em_params* p, const int32_t* bidx, cudaStream_t st) {
   static bool attr_set[SPB_MAX_DEVICES] = {};  // the opt-in is per device (one process may drive several GPUs)
@@ -1484,5 +1763,49 @@ extern "C" int spb_materialize_P(const spb_em_params* p, int32_t iter, float* P,
   materialize_P_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(p->GT, p->ldx, gt_batch_ptr(p, iter), p->colconst, p->XAHat,
                                                                 p->lm, p->sc, p->NA, p->NBb, P, ldp);
   SPB_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int spb_posterior_transfer_rows(const spb_em_params* p, int32_t iter, const float* FB, int64_t ldf, int32_t F,
+                                           float* part, double* out, void* stream) {
+  if (F < 1 || ldf < F || ldf % kXferPanel != 0 || FB == nullptr || part == nullptr || out == nullptr) return SPB_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int32_t* gtb = gt_batch_ptr(p, iter);
+  const int32_t* fb = batch_ptr(p, iter);  // F_B rows are fixed cells (the rows of xb4), whatever the cost matrix's layout
+  for (int f0 = 0; f0 < F; f0 += kXferPanel) {
+    int rc;
+    const float* panel = FB + f0;
+    if (p->sparse_k > 0 && p->D == 2) rc = launch_transfer_rows<true, 2>(p, gtb, fb, panel, ldf, part, st);
+    else if (p->sparse_k > 0) rc = launch_transfer_rows<true, 3>(p, gtb, fb, panel, ldf, part, st);
+    else if (p->D == 2) rc = launch_transfer_rows<false, 2>(p, gtb, fb, panel, ldf, part, st);
+    else rc = launch_transfer_rows<false, 3>(p, gtb, fb, panel, ldf, part, st);
+    if (rc) return rc;
+    SPB_CHECK_LAUNCH();
+    transfer_row_fold_kernel<<<(p->NA + 255) / 256, 256, 0, st>>>(part, p->seg2, p->ldx, p->NA, p->fold_add,
+                                                                   out + (int64_t)f0 * p->ldx);
+    SPB_CHECK_LAUNCH();
+  }
+  return 0;
+}
+
+extern "C" int spb_posterior_transfer_cols(const spb_em_params* p, int32_t iter, const float* FA, int32_t F, float* part,
+                                           float* out, int64_t ldo, void* stream) {
+  if (F < 1 || ldo < F || FA == nullptr || part == nullptr || out == nullptr) return SPB_EINVAL;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int32_t* gtb = gt_batch_ptr(p, iter);
+  for (int f0 = 0; f0 < F; f0 += kXferPanel) {
+    int rc;
+    const float* panel = FA + (int64_t)f0 * p->ldx;
+    if (p->sparse_k > 0 && p->D == 2) rc = launch_transfer_cols<true, 2>(p, gtb, panel, part, st);
+    else if (p->sparse_k > 0) rc = launch_transfer_cols<true, 3>(p, gtb, panel, part, st);
+    else if (p->D == 2) rc = launch_transfer_cols<false, 2>(p, gtb, panel, part, st);
+    else rc = launch_transfer_cols<false, 3>(p, gtb, panel, part, st);
+    if (rc) return rc;
+    SPB_CHECK_LAUNCH();
+    transfer_col_fold_kernel<<<(p->NBb + 127) / 128, 128, 0, st>>>(
+        part, p->keepmask, p->livemask, reinterpret_cast<const int2*>(p->keepoff), (p->nbb_pad + 31) / 32,
+        p->ldx / kRowTile, p->nbb_pad, p->NBb, F - f0 < kXferPanel ? F - f0 : kXferPanel, out + f0, ldo);
+    SPB_CHECK_LAUNCH();
+  }
   return 0;
 }
