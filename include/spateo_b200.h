@@ -339,6 +339,17 @@ int spb_field_geometry(const spb_field_desc* f, const double* X, int64_t n, cons
                        double* torsion, double* div, double* det,
                        void* stream); /* GPVectorField.py:12-125,143-190; gaussian_process.py:102-127 */
 
+/* Trajectories dx/dt = v(x) of n cells through the field f from X0:[n][D] (device doubles), one thread per cell, fp64:
+   scipy.integrate.solve_ivp(v, (0, t_end), x0, method="RK45", max_step, rtol, atol, t_eval=np.linspace(0, t_end, n_out))
+   with dynamo's terminal event np.all(abs(v(x)) < 1e-5) - 1 (morphopath, trajectory.py:11-61, hands the field to
+   dynamo's fate). The sign of t_end is the direction. out[n][n_out][D]: the dense-output samples at the grid times; the
+   samples after a cell's stop hold its state at the stop. t_stop[n]: stop time; steps[n][2]: accepted, rejected steps;
+   status[n]: 0 reached t_end, 1 stopped by the event, -1 failed (100 (n_out - 1) accepted steps, or a step below
+   scipy's minimum). z, Coff: [K][D] device doubles; f is a HOST pointer. No host synchronisation. */
+int spb_field_integrate(const spb_field_desc* f, const double* X0, int64_t n, const double* z, const double* Coff,
+                        double t_end, int32_t n_out, double rtol, double atol, double max_step, double* out,
+                        double* t_stop, int32_t* steps, int32_t* status, void* stream); /* trajectory.py:11-61 */
+
 /* ---- coarse rigid initialisation ---------------------------------------------------------------------------------- */
 /* voxel_data: members of every grid-point ball (radius voxel_size / 2; overlapping) and voxel means. coords [N][D] in
    float (is_f64 = 0) or double, ax0/ax1/ax2 the np.arange axes in the same dtype (device), lo3 / step3 HOST doubles used

@@ -13,6 +13,9 @@ JACOBI="spectrum_and_warm_starts and (clustered-15 or cutoff_straddle-64) or svi
 # sparse top-k select: candidate-cap overflow, ties at tau, subnormals (racecheck / synccheck); 514 row blocks (memcheck)
 SELECT="test_written_cap_ties_subnormals_against_replay and 1024-True"
 MASKOFF="test_mask_off_above_512_row_blocks and 32"
+# trajectory integration: control points tiled through shared memory (block barriers) and the event / step-rejection paths
+PATH_TILED="test_inducing_points_above_the_shared_memory_tile"
+PATH_MEM="test_inducing_points_above_the_shared_memory_tile or test_event_stops or (test_sparsevfc_field and 2)"
 run() {  # tool, pytest args...
   local tool=$1; shift
   echo "=== compute-sanitizer --tool $tool : $*"
@@ -26,16 +29,19 @@ if [ "$TOOL" = memcheck ] || [ "$TOOL" = all ]; then
   run memcheck tests/test_gpu_shard_options.py -k "mapping_from_identical_state or svi_estep_from_identical_state"
   run memcheck tests/test_gpu_mstep.py -k "$MSTEP"
   run memcheck tests/test_gpu_posterior_select.py -k "$MASKOFF"
+  run memcheck tests/test_gpu_morphopath.py -k "$PATH_MEM"
 fi
 if [ "$TOOL" = racecheck ] || [ "$TOOL" = all ]; then
   run racecheck tests/test_gpu_parity.py -k "$NARROW"
   run racecheck tests/test_gpu_gram.py -k "64-7000"
   run racecheck tests/test_gpu_mstep.py -k "$JACOBI"
   run racecheck tests/test_gpu_posterior_select.py -k "$SELECT"
+  run racecheck tests/test_gpu_morphopath.py -k "$PATH_TILED"
 fi
 if [ "$TOOL" = synccheck ] || [ "$TOOL" = all ]; then
   run synccheck tests/test_gpu_parity.py -k "$NARROW"
   run synccheck tests/test_gpu_gram.py -k "64-7000"
   run synccheck tests/test_gpu_mstep.py -k "$JACOBI"
   run synccheck tests/test_gpu_posterior_select.py -k "$SELECT"
+  run synccheck tests/test_gpu_morphopath.py -k "$PATH_TILED"
 fi

@@ -154,6 +154,7 @@ def load_library():
         "spb_rbf_kernel_T": ([P, I64, I64, P, I32, F, P, P], C.c_int),
         "spb_field_eval": ([P, I64, I32, P, P, I32, D, P, P], C.c_int),
         "spb_field_geometry": ([C.POINTER(SpbFieldDesc), P, I64, P, P, P, P, P, P, P, P, P, P, P, P, P], C.c_int),
+        "spb_field_integrate": ([C.POINTER(SpbFieldDesc), P, I64, P, P, D, I32, D, D, D, P, P, P, P, P], C.c_int),
         "spb_voxel_count": ([P, I32, I64, I32, P, I32, P, I32, P, I32, D, P, P, P, P], C.c_int),
         "spb_voxel_accumulate": ([P, I32, I64, I32, P, I32, P, I32, P, I32, D, P, P, P, P, P, I64, I32, P, I64, P], C.c_int),
         "spb_inlier_from_nn": ([P, P, P, I64, I32, D, D, D, D, P, P, P, P, P], C.c_int),

@@ -13,3 +13,4 @@ from .morphofield_dg import (
     morphofield_torsion,
     morphofield_velocity,
 )
+from .morphopath import morphopath
