@@ -256,15 +256,13 @@ int spb_estep_col_select(const spb_em_params* p, int32_t iter, void* stream); /*
 int spb_sparse_P_emit(const spb_em_params* p, int32_t iter, int32_t* rows, float* vals, void* stream); /* utils.py:1385-1392,1506-1510 */
 /* Row / column maxima of the posterior of the last E-step without forming it: rowbest[NA], colbest[NBb] hold
    (float bits of P) << 32 | (0xffffffff - argmax index) — lowest index on ties; either pointer may be NULL.
-   In sparse mode entries below a column's top-k threshold count as absent (0), as in the reference's sparse pi. */
-int spb_posterior_argmax(const spb_em_params* p, int32_t iter, uint64_t* rowbest, uint64_t* colbest,
-                         void* stream); /* spateo/alignment/utils.py:157-191 (get_optimal_mapping_relationship) */
-/* The same with colmap[NBb] (int32, device): the output column index of every column of the E-step, -1 for a column that
-   is not part of the posterior (the row maxima skip it). The row keys then carry colmap[j] instead of j, so a
+   In sparse mode entries below a column's top-k threshold count as absent (0), as in the reference's sparse pi.
+   colmap[NBb] (int32, device; NULL = the identity): the output column index of every column of the E-step, -1 for a column
+   that is not part of the posterior (the row maxima skip it). The row keys carry colmap[j] instead of j, so a
    column-sharded pair passes its block's global column indices and merges the ranks' rowbest with a 64-bit maximum
-   (keys of non-negative values are below 2^63). colbest is unchanged (row indices); NULL colmap = spb_posterior_argmax. */
+   (keys of non-negative values are below 2^63). colbest is unchanged (row indices). */
 int spb_posterior_argmax_mapped(const spb_em_params* p, int32_t iter, const int32_t* colmap, uint64_t* rowbest,
-                                uint64_t* colbest, void* stream);
+                                uint64_t* colbest, void* stream); /* spateo/alignment/utils.py:157-191 (get_optimal_mapping_relationship) */
 int spb_materialize_P(const spb_em_params* p, int32_t iter, float* P, int64_t ldp, void* stream); /* utils.py:1083 */
 /* Posterior transfer of the last E-step without forming P (sparse mode: the entries w >= tau_j, as sweep 2 keeps them).
    Both visit the tiles and quarters of the E-step's work lists, SPB_TRANSFER_PANEL features per pass, no float atomics.

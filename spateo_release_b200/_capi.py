@@ -132,7 +132,6 @@ def load_library():
         "spb_row_stats_p2p": ([EP, I32, C.c_uint64, P], C.c_int),
         "spb_estep_col_select": ([EP, I32, P], C.c_int),
         "spb_sparse_P_emit": ([EP, I32, P, P, P], C.c_int),
-        "spb_posterior_argmax": ([EP, I32, P, P, P], C.c_int),
         "spb_posterior_argmax_mapped": ([EP, I32, P, P, P, P], C.c_int),
         "spb_materialize_P": ([EP, I32, P, I64, P], C.c_int),
         "spb_posterior_transfer_rows": ([EP, I32, P, I64, I32, P, P, P], C.c_int),

@@ -147,9 +147,10 @@ def pair_device_bytes(n_moving: int, n_fixed: int, n_genes: int, chunk_cols: Opt
 
 
 def _room_for_next_pair(dev, need: int) -> bool:
-    """True when ``need`` bytes are free on ``dev``: driver-free memory plus what the caching allocator holds unused."""
-    free, _ = torch.cuda.mem_get_info(dev)
-    return free + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev) >= need
+    """True when ``need`` bytes are free on ``dev`` (``morpho_class._device_budget``)."""
+    from .morpho_class import _device_budget
+
+    return _device_budget(dev) >= need
 
 
 def align_chain_pipelined(
@@ -248,6 +249,28 @@ def align_chain_pipelined(
 def column_block(n_cols: int, rank: int, world: int):
     """Fixed cells [begin, end) of rank ``rank`` when one pair's columns are split over ``world`` GPUs."""
     return (n_cols * rank) // world, (n_cols * (rank + 1)) // world
+
+
+class Collectives:
+    """The exchanges of a column-sharded pair's ranks, on ``torch.distributed``: in place sum and element-wise maximum, and
+    the gather of every rank's per-column rows in rank order. Without a process group of several ranks the sum and the
+    maximum leave ``t`` as it is and the gather returns this rank's own rows. ``m`` is the calling solver; tests that run
+    several shards in one process substitute an object with the same methods that tells the shards apart by it."""
+
+    @staticmethod
+    def _several_ranks() -> bool:
+        return dist.is_initialized() and dist.get_world_size() > 1
+
+    def sum_(self, m, t: torch.Tensor):
+        if self._several_ranks():
+            dist.all_reduce(t)
+
+    def max_(self, m, t: torch.Tensor):
+        if self._several_ranks():
+            dist.all_reduce(t, op=dist.ReduceOp.MAX)
+
+    def gather(self, m, t: torch.Tensor) -> List[torch.Tensor]:
+        return all_gather_rows(t) if self._several_ranks() else [t]
 
 
 def assemble_columns(parts: List[np.ndarray], positions: List[np.ndarray], n_out: int, fill=0) -> np.ndarray:

@@ -1,7 +1,7 @@
 """Optimal cell-to-cell mapping from an alignment posterior (reference: spateo/alignment/utils.py:157-254).
 
 The reference scans a dense ``pi`` on the host (``np.argwhere(pi == pi.max(axis))``). Here the row / column maxima come
-from the device: either from the fused ``spb_posterior_argmax`` kernels, which read the resident cost matrix once and
+from the device: either from the fused ``spb_posterior_argmax_mapped`` kernels, which read the resident cost matrix once and
 never form P (``Morpho_pairwise(..., compute_mapping=True).mapping`` -> :class:`ArgmaxPi`), or — for a dense ``pi`` the
 caller already holds — from chunked torch reductions on the GPU. Ties (several entries equal to the maximum; with
 floating-point posteriors that means an all-zero row or column) are broken with a KD-tree on the coordinates exactly as
@@ -46,7 +46,7 @@ class ArgmaxPi:
 
     @staticmethod
     def decode(keys: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
-        """(argmax, value) from the packed ``spb_posterior_argmax`` keys."""
+        """(argmax, value) from the packed ``spb_posterior_argmax_mapped`` keys."""
         keys = np.asarray(keys, dtype=np.uint64)
         val = (keys >> np.uint64(32)).astype(np.uint32).view(np.float32)
         arg = (np.uint64(0xFFFFFFFF) - (keys & np.uint64(0xFFFFFFFF))).astype(np.int64)

@@ -240,7 +240,9 @@ def shard_svi_schedule(sched: np.ndarray, n_fixed: int, rank: int, world: int):
     of the row is padding: the null column ``c1 - c0`` in ``local`` and -1 in ``pos``. ``w`` is the largest number of
     members any iteration puts in the block (at least 1, so that every launch has a column), so every iteration of the
     rank runs the same E-step launch shape."""
-    c0, c1 = (n_fixed * rank) // world, (n_fixed * (rank + 1)) // world
+    from .distributed import column_block
+
+    c0, c1 = column_block(n_fixed, rank, world)
     inside = (sched >= c0) & (sched < c1)
     width = max(1, int(inside.sum(axis=1).max()))
     local = np.full((sched.shape[0], width), c1 - c0, dtype=np.int32)
@@ -507,6 +509,9 @@ class Morpho_pairwise:
         # column-sharded pair: (rank, world, mode) — this process holds the fixed cells [NB * rank / world, NB * (rank + 1) /
         # world) of ONE pair; see alignment/distributed.py:morpho_align_pair_sharded
         self.column_shard = column_shard
+        from .distributed import Collectives
+
+        self._shard_comm = Collectives()
 
         self._np_dtype = np.float32 if dtype == "float32" else np.float64
         self._check()
@@ -1003,44 +1008,69 @@ class Morpho_pairwise:
         return out
 
     def _build_gene_cost(self):
-        """GT[j][i] = prod_layers prob(metric(A_i, B_j)) (morpho_class.py:265-268 + utils.py:1080-1081)."""
-        dev, lib = self._dev, self._lib
+        """GT[j][i] = prod_layers prob(metric(A_i, B_j)) (morpho_class.py:265-268 + utils.py:1080-1081). Resident: every
+        row is written once, from one layer's operands at a time. Streamed: the operands of every layer are kept for the
+        run, and every iteration refills one [width][ldx] chunk column chunk by column chunk (``_chunk_cost``)."""
+        dev = self._dev
         self._set_row_order()
         c0, c1 = self._col_range()
         nb_loc = c1 - c0
         self._plan_cost(nb_loc)
+        self._gc = GeneCostBuilder(self._lib, dev)
+        specs = list(zip(self.exp_layers_A, self.exp_layers_B, self.dissimilarity, self.probability_type,
+                         self.probability_parameters))
         if self.cost_plan.streamed:
-            self._prepare_streamed_cost()
-            return
-        # an SVI shard pads its iterations to one width with the null column nb_loc: an all-zero cost row
-        self._null_column = self.column_shard is not None and self.SVI_mode
-        self._GT = torch.empty((nb_loc + int(self._null_column), self.ldx), dtype=torch.float32, device=dev)
-        if self._null_column:
-            self._GT[nb_loc:].zero_()
-        gc = GeneCostBuilder(lib, dev)
-        first = True
-        for eA, eB, d_s, p_t, p_p in zip(
-            self.exp_layers_A, self.exp_layers_B, self.dissimilarity, self.probability_type, self.probability_parameters
-        ):
-            if d_s == "label":
-                la = torch.from_numpy(np.ascontiguousarray(eA if self._perm is None else eA[self._perm], dtype=np.int32)).to(dev)
-                lb = torch.from_numpy(np.ascontiguousarray(eB[c0:c1], dtype=np.int32)).to(dev)
-                LT = torch.from_numpy(np.ascontiguousarray(self.label_transfer, dtype=np.float32)).to(dev)
-                check(
-                    lib.spb_label_cost(ptr(la), ptr(lb), ptr(LT), LT.shape[1], self.NA, nb_loc, 0 if first else 1,
-                                       ptr(self._GT), self.ldx, _capi.current_stream_ptr()),
-                    "spb_label_cost",
-                )
-            else:
-                A = self._to_device_pinned(eA)
-                if self._perm is not None:
-                    A = A.index_select(0, self._perm_dev)  # moving cells in Morton order
-                B = self._to_device_pinned(eB) if self.column_shard is None else staged_to_device(eB[c0:c1], dev)
-                opA, rtA, opB, rtB, G_eff = gc.prepare_pair(A, B, d_s)
-                gc.cost(opA, rtA, opB, rtB, self.NA, nb_loc, G_eff, d_s, p_t, p_p, not first, self._GT, self.ldx)
-                del A, B, opA, opB
-            first = False
+            width = self.cost_plan.width
+            self._layers = [self._cost_layer(c0, c1, *spec) for spec in specs]
+            if self.SVI_mode:  # an SVI chunk's fixed-side operands, gathered from its columns every iteration
+                for L in self._layers:
+                    L["g"] = {f: torch.empty((width,) + t.shape[1:], dtype=t.dtype, device=dev) for f, t in L["B"].items()}
+            self._GT = torch.empty((width, self.ldx), dtype=torch.float32, device=dev)
+            self.cost_events = None  # a list: (start, end) CUDA events around the cost of every chunk are appended to it
+        else:
+            # an SVI shard pads its iterations to one width with the null column nb_loc: an all-zero cost row
+            self._null_column = self.column_shard is not None and self.SVI_mode
+            self._GT = torch.empty((nb_loc + int(self._null_column), self.ldx), dtype=torch.float32, device=dev)
+            if self._null_column:
+                self._GT[nb_loc:].zero_()
+            for k, spec in enumerate(specs):
+                self._write_cost(k, self._cost_layer(c0, c1, *spec), 0, nb_loc)
         self.__dict__.pop("_dev_rep", None)  # the resident copies of the representations are no longer needed
+
+    def _cost_layer(self, c0: int, c1: int, eA, eB, d_s, p_t, p_p) -> dict:
+        """Device operands of one layer against this process's fixed cells [c0, c1): the label indices, or the tf32 hi / lo
+        operands of ``GeneCostBuilder.split_pair``. ``B`` holds the fixed side, whose row j is fixed cell c0 + j."""
+        dev = self._dev
+        if d_s == "label":
+            return dict(metric=d_s,
+                        la=torch.from_numpy(np.ascontiguousarray(self._sorted(eA), dtype=np.int32)).to(dev),
+                        LT=torch.from_numpy(np.ascontiguousarray(self.label_transfer, dtype=np.float32)).to(dev),
+                        B=dict(lb=torch.from_numpy(np.ascontiguousarray(eB[c0:c1], dtype=np.int32)).to(dev)))
+        A = self._to_device_pinned(eA)
+        if self._perm is not None:
+            A = A.index_select(0, self._perm_dev)  # moving cells in processing order
+        B = self._to_device_pinned(eB) if self.column_shard is None else staged_to_device(eB[c0:c1], dev)
+        L = self._gc.split_pair(*self._gc.prepare_pair(A, B, d_s))
+        fixed = {f: L.pop(f) for f in ("bhi", "blo", "rtB")}
+        L.update(metric=d_s, p_t=p_t, p_p=p_p, B={f: t for f, t in fixed.items() if t is not None})
+        return L
+
+    def _write_cost(self, k: int, L: dict, c0: int, c1: int, idx: Optional[torch.Tensor] = None):
+        """Cost rows of layer ``k`` (operands ``L`` of ``_cost_layer``) into ``_GT``: row j from the fixed-side row c0 + j,
+        or, given ``idx`` (an SVI chunk's columns), from row idx[j], gathered first. Layer 0 writes, later layers multiply."""
+        n = c1 - c0
+        if idx is None:
+            B = {f: t[c0:c1] for f, t in L["B"].items()}
+        else:
+            B = L["g"]
+            for f, t in L["B"].items():
+                self._gather(t, idx, n, B[f])
+        if L["metric"] == "label":
+            check(self._lib.spb_label_cost(ptr(L["la"]), ptr(B["lb"]), ptr(L["LT"]), L["LT"].shape[1], self.NA, n, int(k > 0),
+                                           ptr(self._GT), self.ldx, _capi.current_stream_ptr()), "spb_label_cost")
+        else:
+            self._gc.cost_split(L["ahi"], L["alo"], L["rtA"], B["bhi"], B["blo"], B.get("rtB"), self.NA, n, L["G"],
+                                L["metric"], L["p_t"], L["p_p"], k > 0, self._GT, self.ldx)
 
     def _cost_features(self) -> int:
         """Features of the expression operands of all layers together (sym_kl contracts over both of its halves)."""
@@ -1080,42 +1110,6 @@ class Morpho_pairwise:
         plan = getattr(self, "cost_plan", None)
         return plan is not None and plan.streamed
 
-    def _prepare_streamed_cost(self):
-        """Streamed cost matrix: the operands of every layer, split into tf32 hi / lo once and kept for the run, and one
-        [width][ldx] chunk that every iteration refills column chunk by column chunk (``_chunk_cost``)."""
-        dev, lib = self._dev, self._lib
-        width = self.cost_plan.width
-        gc = GeneCostBuilder(lib, dev)
-        self._gc, self._layers = gc, []
-        for eA, eB, d_s, p_t, p_p in zip(
-            self.exp_layers_A, self.exp_layers_B, self.dissimilarity, self.probability_type, self.probability_parameters
-        ):
-            if d_s == "label":
-                L = dict(
-                    kind="label",
-                    la=torch.from_numpy(np.ascontiguousarray(eA if self._perm is None else eA[self._perm], dtype=np.int32)).to(dev),
-                    lb=torch.from_numpy(np.ascontiguousarray(eB, dtype=np.int32)).to(dev),
-                    LT=torch.from_numpy(np.ascontiguousarray(self.label_transfer, dtype=np.float32)).to(dev),
-                )
-                if self.SVI_mode:
-                    L["lb_g"] = torch.empty((width,), dtype=torch.int32, device=dev)
-            else:
-                A = self._to_device_pinned(eA)
-                if self._perm is not None:
-                    A = A.index_select(0, self._perm_dev)
-                B = self._to_device_pinned(eB)
-                L = gc.split_pair(*gc.prepare_pair(A, B, d_s))
-                del A, B
-                L.update(kind="tc", metric=d_s, p_t=p_t, p_p=p_p)
-                if self.SVI_mode:
-                    L["g"] = dict(bhi=torch.empty((width, L["bhi"].shape[1]), dtype=torch.float32, device=dev),
-                                  blo=torch.empty((width, L["blo"].shape[1]), dtype=torch.float32, device=dev),
-                                  rtB=None if L["rtB"] is None else torch.empty((width,), dtype=torch.float32, device=dev))
-            self._layers.append(L)
-        self.__dict__.pop("_dev_rep", None)
-        self._GT = torch.empty((width, self.ldx), dtype=torch.float32, device=dev)
-        self.cost_events = None  # a list: (start, end) CUDA events around the cost of every chunk are appended to it
-
     def _gather(self, src: torch.Tensor, idx: torch.Tensor, n: int, dst: torch.Tensor):
         """dst[:n] = src[idx[:n]] (rows of 4-byte words) on the device."""
         width = src.shape[1] if src.dim() == 2 else 1
@@ -1128,43 +1122,23 @@ class Morpho_pairwise:
         """Cost rows of one column chunk into ``_GT`` (row j = column c0 + j of the iteration): the fixed cells [c0, c1)
         when ``idx`` is None, else the fixed cells ``idx`` (this iteration's row of the chunk's SVI schedule), whose
         operands are gathered first."""
-        lib, NA, ldx, st = self._lib, self.NA, self.ldx, _capi.current_stream_ptr()
-        n = c1 - c0
         ev = self.cost_events
         if ev is not None:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
         for k, L in enumerate(self._layers):
-            if L["kind"] == "label":
-                lb = L["lb"][c0:c1]
-                if idx is not None:
-                    self._gather(L["lb"], idx, n, L["lb_g"])
-                    lb = L["lb_g"]
-                check(lib.spb_label_cost(ptr(L["la"]), ptr(lb), ptr(L["LT"]), L["LT"].shape[1], NA, n, 1 if k else 0,
-                                         ptr(self._GT), ldx, st), "spb_label_cost")
-                continue
-            if idx is None:
-                bhi, blo = L["bhi"][c0:c1], L["blo"][c0:c1]
-                rtB = None if L["rtB"] is None else L["rtB"][c0:c1]
-            else:
-                g = L["g"]
-                self._gather(L["bhi"], idx, n, g["bhi"])
-                self._gather(L["blo"], idx, n, g["blo"])
-                if g["rtB"] is not None:
-                    self._gather(L["rtB"], idx, n, g["rtB"])
-                bhi, blo, rtB = g["bhi"], g["blo"], g["rtB"]
-            self._gc.cost_split(L["ahi"], L["alo"], L["rtA"], bhi, blo, rtB, NA, n, L["G"], L["metric"], L["p_t"], L["p_p"],
-                                k > 0, self._GT, ldx)
+            self._write_cost(k, L, c0, c1, idx)
         if ev is not None:
             e1.record()
             ev.append((e0, e1))
 
     def _col_range(self):
         """Fixed cells (columns of P) held by this process: all of them, or this rank's block of a column-sharded pair."""
+        from .distributed import column_block
+
         if self.column_shard is None:
             return 0, self.NB
-        r, w = int(self.column_shard[0]), int(self.column_shard[1])
-        return (self.NB * r) // w, (self.NB * (r + 1)) // w
+        return column_block(self.NB, int(self.column_shard[0]), int(self.column_shard[1]))
 
     def _to_device_pinned(self, host_array: np.ndarray) -> torch.Tensor:
         """Device copy of one dense representation, uploaded ONCE per preparation (the coarse initialisation, the beta^2
@@ -1276,9 +1250,8 @@ class Morpho_pairwise:
         s["livemask"] = torch.zeros_like(s["keepmask"])
         s["keepoff"] = torch.zeros((nrb, (self._nbb_pad + 31) // 32, 2), dtype=torch.int32, device=dev)
         n_sms = torch.cuda.get_device_properties(dev).multi_processor_count
-        seg1 = self._choose_segments(nrb, min(nbb, width), n_sms)
-        seg2 = self._choose_segments(nrb, min(nbb, width), n_sms)
-        seg_alloc = max(seg2, self._choose_segments(nrb, width, n_sms))
+        seg = self._choose_segments(nrb, min(nbb, width), n_sms)  # column segments of both sweeps
+        seg_alloc = max(seg, self._choose_segments(nrb, width, n_sms))
         s["rowpart"] = torch.zeros((seg_alloc, 8, ldx), dtype=f32, device=dev)
         s["bbox"] = torch.zeros((nrb, 4, 8), dtype=f32, device=dev)
         s["collist"] = torch.zeros((nrb, self._nbb_pad), dtype=torch.int32, device=dev)
@@ -1316,6 +1289,7 @@ class Morpho_pairwise:
         host_sc = np.frombuffer(bytes(sc), dtype=np.uint8).copy()
         s["sc"] = torch.from_numpy(host_sc).to(dev)
         self._state = s
+        self._P_captured = False  # set by _capture_begin: this state's final posterior has been captured
         self.__dict__.pop("_graphs", None)  # captured iteration graphs hold the old state's pointers
         # params
         p = SpbEmParams()
@@ -1335,7 +1309,7 @@ class Morpho_pairwise:
             p.rowstat = s["rowstat"].data_ptr()
         p.svi, p.nn_init, p.update_R = int(self.SVI_mode), int(self.nn_init), int(self.update_R)
         p.nonrigid_start_iter = int(self.nonrigid_start_iter)
-        p.seg1, p.seg2, p.nbb_pad, p.trace = seg1, seg2, self._nbb_pad, 1
+        p.seg1, p.seg2, p.nbb_pad, p.trace = seg, seg, self._nbb_pad, 1
         p.cull = int(bool(self.cull_zero_tiles))
         p.sparse_k = int(self.sparse_top_k) if self.sparse_calculation_mode else 0
         p.lambdaVF, p.gamma_a, p.gamma_b = float(self.lambdaVF), float(self.gamma_a), float(self.gamma_b)
@@ -1461,8 +1435,8 @@ class Morpho_pairwise:
         s = self._state
         if self._FB_host is not None:
             acc = s["xfer_PFB"]
-            if self.column_shard is not None:
-                self._shard_sum_tensor(acc)
+            if self.column_shard is not None:  # the collective, whatever sums the row statistics
+                self._shard_comm.sum_(self, acc)
             pfb = acc[: self._FB_host.shape[1], : self.NA].T.contiguous().to(torch.float32)
             _count_d2h(pfb)
             self.P_FB = self._unsorted(pfb.cpu().numpy())
@@ -1528,26 +1502,7 @@ class Morpho_pairwise:
             check(self._lib.spb_row_stats_p2p(C.byref(self._params), (self._shard_epoch - 1) & 1, self._shard_epoch, st),
                   "spb_row_stats_p2p")
             return
-        comm = getattr(self, "_shard_comm", None)
-        if comm is not None:  # tests: several shards of one process, each driven by its own thread
-            comm.sum_(self, view)
-        else:
-            import torch.distributed as dist
-
-            if dist.is_initialized() and dist.get_world_size() > 1:
-                dist.all_reduce(view)
-
-    def _shard_sum_tensor(self, t: torch.Tensor):
-        """In place: the sum of every rank's fp64 ``t`` through the collective, whatever the row-statistics mode (the
-        peer-memory kernel sums only those)."""
-        comm = getattr(self, "_shard_comm", None)
-        if comm is not None:
-            comm.sum_(self, t)
-        else:
-            import torch.distributed as dist
-
-            if dist.is_initialized() and dist.get_world_size() > 1:
-                dist.all_reduce(t)
+        self._shard_comm.sum_(self, view)
 
     def _shard_finish_rows(self, st):
         """Finish the row statistics from the view of ``_shard_fold`` once ``_shard_sum`` made it the sum over the ranks
@@ -1561,32 +1516,6 @@ class Morpho_pairwise:
         """Row statistics of a column-sharded pair: local fold, sum over the ranks, finish (replaces spb_row_finalize)."""
         self._shard_sum(self._shard_fold(st), st)
         self._shard_finish_rows(st)
-
-    def _shard_gather(self, t: torch.Tensor) -> list:
-        """Every rank's ``t`` (per-column rows of its E-step columns), in rank order; only this rank's own without a
-        process group."""
-        comm = getattr(self, "_shard_comm", None)
-        if comm is not None:
-            return comm.gather(self, t)
-        import torch.distributed as dist
-
-        if dist.is_initialized() and dist.get_world_size() > 1:
-            from .distributed import all_gather_rows
-
-            return all_gather_rows(t)
-        return [t]
-
-    def _shard_max_(self, keys: torch.Tensor) -> torch.Tensor:
-        """In place: the element-wise maximum of every rank's int64 ``keys`` (argmax keys of non-negative values)."""
-        comm = getattr(self, "_shard_comm", None)
-        if comm is not None:
-            comm.max_(self, keys)
-        else:
-            import torch.distributed as dist
-
-            if dist.is_initialized() and dist.get_world_size() > 1:
-                dist.all_reduce(keys, op=dist.ReduceOp.MAX)
-        return keys
 
     def _shard_positions(self) -> list:
         """Output column of every E-step column of every rank, in rank order (-1: null column): batch positions for an SVI
@@ -1609,7 +1538,7 @@ class Morpho_pairwise:
         ([n_out, ...]; null columns dropped). Without a process group only this rank's columns are returned."""
         from .distributed import assemble_columns
 
-        parts = [q.cpu().numpy() for q in self._shard_gather(t)]
+        parts = [q.cpu().numpy() for q in self._shard_comm.gather(self, t)]
         pos = self._shard_positions()
         if len(parts) == 1 and len(pos) > 1:  # no collective: this rank's own columns
             mine = pos[int(self.column_shard[0])]
@@ -1659,27 +1588,25 @@ class Morpho_pairwise:
         rank = s.setdefault("sigma_rank", torch.zeros((1,), dtype=torch.int32, device=self._dev))
         rank.copy_((keep & (ev > 0)).sum().to(torch.int32).reshape(1))
 
+    def _fusable(self, it: int) -> bool:
+        """Iteration ``it`` can run as the fused single call and be replayed from a CUDA graph: a resident, unsharded pair,
+        outside the non-rigid phase of K > SPB_MAX_K_FUSED (eigen solve through cuSOLVER)."""
+        large_K = it > self.nonrigid_start_iter and self.K > _capi.MAX_K_FUSED
+        return not (large_K or self.column_shard is not None or self._streamed)
+
     def _iteration(self, it: int, st, capture_P: bool = False, sweep_events: Optional[list] = None):
         """One EM iteration (morpho_class.py:280-294). The fused C entry point is used unless the iteration has to be
-        split: K > SPB_MAX_K_FUSED (eigen solve through cuSOLVER) or ``capture_P`` (dense P of THIS E-step, which must
-        be written before the M-step moves the cells)."""
-        lib, p = self._lib, self._params
-        nonrigid = it > self.nonrigid_start_iter
-        large_K = nonrigid and self.K > _capi.MAX_K_FUSED
-        if not (large_K or capture_P or sweep_events is not None or self.column_shard is not None or self._streamed):
-            check(lib.spb_em_iteration(C.byref(p), it, st), "spb_em_iteration")
+        split: it is not ``_fusable``, it records ``sweep_events``, or it captures the posterior of THIS E-step
+        (``capture_P``), which must be read before the M-step moves the cells."""
+        if self._fusable(it) and not capture_P and sweep_events is None:
+            check(self._lib.spb_em_iteration(C.byref(self._params), it, st), "spb_em_iteration")
             return
-        if self.column_shard is not None:  # (a column-sharded pair is never streamed)
+        if self.column_shard is not None:
             view = self._shard_iteration_local(it, st, capture_P, sweep_events)
             self._shard_sum(view, st)
             self._shard_iteration_finish(it, st)
             return
-        if self._streamed:
-            self._estep_only(it, st, on_chunk=self._streamed_capture() if capture_P else None)
-        else:
-            self._estep_only(it, st, sweep_events)
-            if capture_P:
-                self._capture_P(it, st)
+        self._estep_only(it, st, sweep_events, on_chunk=self._capture_begin() if capture_P else None)
         self._mstep(it, st)
 
     def _shard_iteration_local(self, it: int, st, capture_P: bool = False,
@@ -1687,9 +1614,7 @@ class Morpho_pairwise:
         """First half of a column-sharded iteration: the E-step of this rank's columns (and the posterior capture of the
         last iteration) up to the fold of its row statistics. Returns the fp64 view that ``_shard_sum`` sums over the ranks
         before ``_shard_iteration_finish`` (``_iteration`` runs the three in this order)."""
-        self._estep_local(it, st, sweep_events)
-        if capture_P:
-            self._capture_P(it, st)
+        self._estep_local(it, st, sweep_events, on_chunk=self._capture_begin() if capture_P else None)
         return self._shard_fold(st)
 
     def _shard_iteration_finish(self, it: int, st):
@@ -1717,33 +1642,49 @@ class Morpho_pairwise:
         check(lib.spb_rigid_solve(C.byref(p), it, st), "spb_rigid_solve")
         check(lib.spb_row_update(C.byref(p), st), "spb_row_update")
 
-    def _capture_P(self, it: int, st):
-        """Posterior of the E-step that has just run: dense [N_A, NBb], or in sparse_calculation_mode the COO entries
-        (top-k rows and values per column) without ever forming the dense matrix."""
-        lib, p = self._lib, self._params
+    def _capture_begin(self):
+        """Outputs of the posterior capture of the E-step about to run (``_NBb`` columns): P @ F_B / P^T @ F_A, the argmax
+        keys, and the dense P or, in sparse_calculation_mode, its COO entries (top-k rows and values per column), as the
+        options ask. Returns ``_capture_chunk``, the ``on_chunk`` hook of ``_estep_only`` that fills them."""
+        dev, n = self._dev, self._NBb
         if self._transfer_on:
             self._transfer_begin()
-            self._transfer_capture(p, it, st)
         if self.compute_mapping:  # row / column maxima of the same posterior, straight from the cost matrix
-            self._rowbest = torch.zeros((self.NA,), dtype=torch.int64, device=self._dev)
-            self._colbest = torch.zeros((self._NBb,), dtype=torch.int64, device=self._dev)
-            colmap = None
+            self._rowbest = torch.zeros((self.NA,), dtype=torch.int64, device=dev)
+            self._colbest = torch.zeros((n,), dtype=torch.int64, device=dev)
+            self._colmap = None
             if self.column_shard is not None:  # row keys carry the unsharded column index; null columns are skipped
-                colmap = torch.from_numpy(self._shard_positions()[int(self.column_shard[0])]).to(self._dev)
-            check(lib.spb_posterior_argmax_mapped(C.byref(p), it, ptr(colmap), ptr(self._rowbest), ptr(self._colbest), st),
-                  "spb_posterior_argmax_mapped")
-        if not self.materialize_P:
-            self._P_dev = "skipped"
-            return
-        if self.sparse_calculation_mode:
+                self._colmap = torch.from_numpy(self._shard_positions()[int(self.column_shard[0])]).to(dev)
+        if self.materialize_P and self.sparse_calculation_mode:
             k = int(self.sparse_top_k)
-            self._P_rows = torch.zeros((self._NBb, k), dtype=torch.int32, device=self._dev)
-            self._P_vals = torch.zeros((self._NBb, k), dtype=torch.float32, device=self._dev)
-            check(lib.spb_sparse_P_emit(C.byref(p), it, ptr(self._P_rows), ptr(self._P_vals), st), "spb_sparse_P_emit")
-            self._P_dev = "sparse"
-        else:
-            self._P_dev = torch.empty((self.NA, self._NBb), dtype=torch.float32, device=self._dev)
-            check(lib.spb_materialize_P(C.byref(p), it, ptr(self._P_dev), self._NBb, st), "spb_materialize_P")
+            self._P_rows = torch.zeros((n, k), dtype=torch.int32, device=dev)
+            self._P_vals = torch.zeros((n, k), dtype=torch.float32, device=dev)
+        elif self.materialize_P:
+            self._P_dev = torch.empty((self.NA, n), dtype=torch.float32, device=dev)
+        self._P_captured = True
+        return self._capture_chunk
+
+    def _capture_chunk(self, q: SpbEmParams, it: int, c0: int, c1: int, st=None):
+        """The posterior of the E-step columns [c0, c1) that ``q`` describes, while their lists and column constants are
+        live, launched on ``st`` (default: the current stream, on which ``on_chunk`` runs). The argmax keys and the dense P
+        are only captured from a whole E-step: a streamed pair, the only one whose E-step comes in several chunks, refuses
+        both (``_plan_cost``)."""
+        lib = self._lib
+        st = _capi.current_stream_ptr() if st is None else st
+        if self._transfer_on:
+            self._transfer_capture(q, it, st, c0)
+        if self.compute_mapping:
+            check(lib.spb_posterior_argmax_mapped(C.byref(q), it, ptr(self._colmap), ptr(self._rowbest), ptr(self._colbest),
+                                                  st), "spb_posterior_argmax_mapped")
+        if self.materialize_P and self.sparse_calculation_mode:
+            check(lib.spb_sparse_P_emit(C.byref(q), it, ptr(self._P_rows[c0:c1]), ptr(self._P_vals[c0:c1]), st),
+                  "spb_sparse_P_emit")
+        elif self.materialize_P:
+            check(lib.spb_materialize_P(C.byref(q), it, ptr(self._P_dev), self._NBb, st), "spb_materialize_P")
+
+    def _capture_P(self, it: int, st):
+        """Capture the posterior of the whole E-step that has just run (``_capture_begin`` + ``_capture_chunk``)."""
+        self._capture_begin()(self._params, it, 0, self._NBb, st)
 
     def _sparse_P_to_coo(self, dt, P_rows: Optional[torch.Tensor] = None, P_vals: Optional[torch.Tensor] = None):
         """scipy COO in the reference's layout (utils.py:1385-1392,1506-1510) from the [n_cols][sparse_top_k] entries of
@@ -1764,34 +1705,61 @@ class Morpho_pairwise:
         return sp.coo_matrix((vals.cpu().numpy().astype(dt).reshape(-1), (rows.reshape(-1), col)), shape=(self.NA, n_cols))
 
     def _estep_only(self, it: int, st, sweep_events: Optional[list] = None, on_chunk=None):
-        """One E-step + the statistics the closing similarity needs (used for return_mapping under SVI)."""
+        """One E-step + its row statistics, which the M-step and the closing similarity read (``_estep_local``)."""
+        lib, p = self._lib, self._params
+        self._estep_local(it, st, sweep_events, on_chunk)
         if self._streamed:
-            self._estep_streamed(it, st, on_chunk)
-            return
-        self._estep_local(it, st, sweep_events)
-        if self.column_shard is not None:
+            check(lib.spb_row_stats_finalize(C.byref(p), 0, st), "spb_row_stats_finalize")
+        elif self.column_shard is not None:
             self._shard_row_statistics(st)
         else:
-            check(self._lib.spb_row_finalize(C.byref(self._params), st), "spb_row_finalize")
+            check(lib.spb_row_finalize(C.byref(p), st), "spb_row_finalize")
 
-    def _estep_local(self, it: int, st, sweep_events: Optional[list] = None):
-        """The E-step of a resident cost matrix up to its row partials (sweep 2)."""
-        lib, p = self._lib, self._params
+    def _estep_local(self, it: int, st, sweep_events: Optional[list] = None, on_chunk=None):
+        """The E-step of this process's columns up to its row partials (sweep 2). A streamed cost matrix is recomputed
+        chunk by chunk: per chunk the cost rows, then the sweeps, whose row partials are folded into the fp64 row statistics
+        in chunk order (reproducible). ``on_chunk(params, it, c0, c1)`` runs after every sweep 2, while its cost rows and
+        column constants are live: once with ``_params`` over all columns, or once per chunk [c0, c1) of a streamed E-step.
+        ``sweep_events`` receives the events of ``_estep_sweeps`` (not recorded for a streamed E-step)."""
+        lib, p, s = self._lib, self._params, self._state
         check(lib.spb_iter_begin(C.byref(p), it, st), "spb_iter_begin")
-        check(lib.spb_gather_cols(C.byref(p), it, st), "spb_gather_cols")
-        check(lib.spb_estep_col_lists(C.byref(p), st), "spb_estep_col_lists")
+        if not self._streamed:
+            self._estep_sweeps(p, it, st, sweep_events)
+            if on_chunk is not None:
+                on_chunk(p, it, 0, p.NBb)
+            return
+        cols, width = p.NBb, self.cost_plan.width
+        for k, c0 in enumerate(range(0, cols, width)):
+            c1 = min(cols, c0 + width)
+            q = self._chunk_params(k, c0, c1)
+            q.fold_add = int(k > 0)
+            self._chunk_cost(c0, c1, s["chunk_sched"][k][it] if p.svi else None)
+            if c1 - c0 < width:  # ragged chunk: the pad column record after the last column is zero, as in a full one
+                s["colgeom"][c1 - c0:].zero_()
+                s["colconst"][c1 - c0:].zero_()
+            self._estep_sweeps(q, it, st)
+            if on_chunk is not None:
+                on_chunk(q, it, c0, c1)
+            check(lib.spb_row_fold(C.byref(q), 0, st), "spb_row_fold")
+
+    def _estep_sweeps(self, q: SpbEmParams, it: int, st, sweep_events: Optional[list] = None):
+        """The E-step launches of the columns ``q`` describes, from the column gather to sweep 2. ``sweep_events``: a list
+        that receives (start, after sweep 1, before sweep 2, end) CUDA events."""
+        lib, qp = self._lib, C.byref(q)
+        check(lib.spb_gather_cols(qp, it, st), "spb_gather_cols")
+        check(lib.spb_estep_col_lists(qp, st), "spb_estep_col_lists")
         if sweep_events is not None:
             e0, e1, e2, e3 = (torch.cuda.Event(enable_timing=True) for _ in range(4))
             e0.record()
-        check(lib.spb_estep_sweep1(C.byref(p), it, st), "spb_estep_sweep1")
+        check(lib.spb_estep_sweep1(qp, it, st), "spb_estep_sweep1")
         if sweep_events is not None:
             e1.record()
-        check(lib.spb_col_finalize(C.byref(p), st), "spb_col_finalize")
+        check(lib.spb_col_finalize(qp, st), "spb_col_finalize")
         if self.sparse_calculation_mode:
-            check(lib.spb_estep_col_select(C.byref(p), it, st), "spb_estep_col_select")
+            check(lib.spb_estep_col_select(qp, it, st), "spb_estep_col_select")
         if sweep_events is not None:
             e2.record()
-        check(lib.spb_estep_sweep2(C.byref(p), it, st), "spb_estep_sweep2")
+        check(lib.spb_estep_sweep2(qp, it, st), "spb_estep_sweep2")
         if sweep_events is not None:
             e3.record()
             sweep_events.append((e0, e1, e2, e3))
@@ -1811,64 +1779,6 @@ class Morpho_pairwise:
             q.batch_idx = None
             q.xb4 = s["xb4"].data_ptr() + 16 * c0
         return q
-
-    def _estep_streamed(self, it: int, st, on_chunk=None):
-        """One E-step with the cost matrix recomputed chunk by chunk: per chunk the cost rows, then the E-step pieces up to
-        sweep 2, whose row partials are folded into the fp64 row statistics in chunk order (reproducible); the statistics are
-        finished once. ``on_chunk(params, it, c0, c1)`` runs after a chunk's sweep 2, while its cost rows and column constants
-        are live."""
-        lib, p, s = self._lib, self._params, self._state
-        check(lib.spb_iter_begin(C.byref(p), it, st), "spb_iter_begin")
-        cols, width = p.NBb, self.cost_plan.width
-        for k, c0 in enumerate(range(0, cols, width)):
-            c1 = min(cols, c0 + width)
-            q = self._chunk_params(k, c0, c1)
-            q.fold_add = int(k > 0)
-            self._chunk_cost(c0, c1, s["chunk_sched"][k][it] if p.svi else None)
-            if c1 - c0 < width:  # ragged chunk: the pad column record after the last column is zero, as in a full one
-                s["colgeom"][c1 - c0:].zero_()
-                s["colconst"][c1 - c0:].zero_()
-            qp = C.byref(q)
-            check(lib.spb_gather_cols(qp, it, st), "spb_gather_cols")
-            check(lib.spb_estep_col_lists(qp, st), "spb_estep_col_lists")
-            check(lib.spb_estep_sweep1(qp, it, st), "spb_estep_sweep1")
-            check(lib.spb_col_finalize(qp, st), "spb_col_finalize")
-            if self.sparse_calculation_mode:
-                check(lib.spb_estep_col_select(qp, it, st), "spb_estep_col_select")
-            check(lib.spb_estep_sweep2(qp, it, st), "spb_estep_sweep2")
-            if on_chunk is not None:
-                on_chunk(q, it, c0, c1)
-            check(lib.spb_row_fold(qp, 0, st), "spb_row_fold")
-        check(lib.spb_row_stats_finalize(C.byref(p), 0, st), "spb_row_stats_finalize")
-
-    def _streamed_capture(self):
-        """Posterior capture of a streamed E-step, run on every chunk while it is live: the COO entries of its columns
-        (sparse mode) and the posterior transfer; None when nothing is captured."""
-        hooks = []
-        if self.materialize_P and self.sparse_calculation_mode:
-            k = int(self.sparse_top_k)
-            self._P_rows = torch.zeros((self._NBb, k), dtype=torch.int32, device=self._dev)
-            self._P_vals = torch.zeros((self._NBb, k), dtype=torch.float32, device=self._dev)
-            self._P_dev = "sparse"
-
-            def emit(q, it, c0, c1):
-                check(self._lib.spb_sparse_P_emit(C.byref(q), it, ptr(self._P_rows[c0:c1]), ptr(self._P_vals[c0:c1]),
-                                                  _capi.current_stream_ptr()), "spb_sparse_P_emit")
-
-            hooks.append(emit)
-        else:
-            self._P_dev = "skipped"
-        if self._transfer_on:
-            self._transfer_begin()
-            hooks.append(lambda q, it, c0, c1: self._transfer_capture(q, it, _capi.current_stream_ptr(), c0))
-        if not hooks:
-            return None
-
-        def capture(q, it, c0, c1):
-            for h in hooks:
-                h(q, it, c0, c1)
-
-        return capture
 
     def prepare_host(self):
         """Coarse rigid initialisation + variational initialisation (host numpy with small device helpers); consumes
@@ -1930,9 +1840,7 @@ class Morpho_pairwise:
                 last = it == self.max_iter - 1
                 want_P = self._captures_posterior and last and not (self.return_mapping and self.SVI_mode)
                 nonrigid = it > self.nonrigid_start_iter
-                plain = (hist is not None or sweep_events is not None or want_P or self.column_shard is not None
-                         or self._streamed or (nonrigid and self.K > _capi.MAX_K_FUSED))
-                if not plain:
+                if not (hist is not None or sweep_events is not None or want_P or not self._fusable(it)):
                     # iterations [it, stop) share the phase and need nothing from the host
                     stop = min(end, self.nonrigid_start_iter + 1) if not nonrigid else end
                     if self._captures_posterior and stop == self.max_iter and not (self.return_mapping and self.SVI_mode):
@@ -2026,12 +1934,10 @@ class Morpho_pairwise:
             s["sc"].copy_(torch.from_numpy(np.frombuffer(bytes(sc), dtype=np.uint8).copy()))
             check(lib.spb_row_update(C.byref(p), st), "spb_row_update")
         full_mapping = self.return_mapping and self.SVI_mode
-
-        def capture():  # a streamed E-step captures the posterior while its chunks are live
-            return self._streamed_capture() if self._streamed and getattr(self, "_P_dev", None) is None else None
-
+        # the closing E-step (max_iter == 0, or the full posterior of return_mapping) is the one whose posterior is captured
+        capture = self._captures_posterior
         if self.max_iter == 0:
-            self._estep_only(0, st, on_chunk=None if full_mapping else capture())
+            self._estep_only(0, st, on_chunk=self._capture_begin() if capture and not full_mapping else None)
             check(lib.spb_rigid_moments(C.byref(p), st), "spb_rigid_moments")
         if full_mapping:
             # full (non-SVI) posterior with the final parameters (morpho_class.py:300-302)
@@ -2044,7 +1950,7 @@ class Morpho_pairwise:
                 p.seg1 = p.seg2 = self._choose_segments(self.ldx // _capi.ROW_TILE, nb,
                                                         torch.cuda.get_device_properties(self._dev).multi_processor_count)
             self._NBb = nb
-            self._estep_only(last_iter, st, on_chunk=capture())
+            self._estep_only(last_iter, st, on_chunk=self._capture_begin() if capture else None)
             # scalar Sp's must become the un-averaged sums (morpho_class.py:1183-1185)
             sc = self._read_scalars()
             sc.Sp_spatial, sc.Sp_sigma2, sc.Sp = sc.sums[0], sc.sums[1], sc.sums[2]
@@ -2093,8 +1999,8 @@ class Morpho_pairwise:
         else:
             self.Coff = np.zeros(self.K, dtype=dt)  # the reference's initial value (morpho_class.py:733)
         self.trace = s["trace_buf"].cpu().numpy()
-        if self._captures_posterior and getattr(self, "_P_dev", None) is None:
-            self._capture_P(last_iter, st)  # max_iter == 0 or the return_mapping E-step above
+        if capture and not self._P_captured:  # run_em stopped before the last iteration: the E-step that ran last
+            self._capture_P(last_iter, st)
         if self._transfer_on:
             self._transfer_results(n_cols)
         if self.compute_mapping:
@@ -2102,14 +2008,15 @@ class Morpho_pairwise:
 
             rowbest, colbest = self._rowbest.cpu().numpy(), self._colbest.cpu().numpy()
             if self.column_shard is not None:  # row keys: the largest over the ranks; column keys: gathered
-                rowbest = self._shard_max_(self._rowbest).cpu().numpy()
+                self._shard_comm.max_(self, self._rowbest)
+                rowbest = self._rowbest.cpu().numpy()
                 colbest = self._shard_columns(self._colbest, n_cols)
             ra, rv = ArgmaxPi.decode(rowbest.view(np.uint64))
             ca, cv = ArgmaxPi.decode(colbest.view(np.uint64))
             if self._perm is not None:  # device rows are in processing order
                 ra, rv, ca = self._unsorted(ra), self._unsorted(rv), self._perm[ca]
             self.mapping = ArgmaxPi((NA, colbest.shape[0]), ra, rv.astype(dt), ca, cv.astype(dt))
-            self._rowbest = self._colbest = None
+            self._rowbest = self._colbest = self._colmap = None
         if self.materialize_P:
             if self.sparse_calculation_mode:
                 rows, vals = self._P_rows, self._P_vals
@@ -2123,7 +2030,7 @@ class Morpho_pairwise:
                 self.P = self._unsorted(self._P_dev.cpu().numpy().astype(dt))
         else:
             self.P = None
-        self._P_dev = None
+        self._P_dev, self._P_captured = None, False
         if self.iter_key_added is not None:
             hist_d = s["hist"][:, :D, :NA].permute(0, 2, 1).contiguous()
             _count_d2h(hist_d)

@@ -1694,11 +1694,6 @@ extern "C" int spb_sparse_P_emit(const spb_em_params* p, int32_t iter, int32_t* 
   return 0;
 }
 
-extern "C" int spb_posterior_argmax(const spb_em_params* p, int32_t iter, uint64_t* rowbest, uint64_t* colbest,
-                                    void* stream) {
-  return spb_posterior_argmax_mapped(p, iter, nullptr, rowbest, colbest, stream);
-}
-
 extern "C" int spb_posterior_argmax_mapped(const spb_em_params* p, int32_t iter, const int32_t* colmap, uint64_t* rowbest,
                                            uint64_t* colbest, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;

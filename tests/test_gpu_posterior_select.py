@@ -483,18 +483,18 @@ def test_mask_off_above_512_row_blocks(k):
 def test_streamed_ragged_chunks_against_replay(monkeypatch, golden):
     """3d_full_warp streamed in three column chunks, the last one shorter: per chunk, tau and the COO against the replay
     of the chunk's weights; the folded row sums against the sum of the chunks' replays."""
-    from test_gpu_streamed_cost import _force_width, _three_chunks
+    from layout_helpers import force_width, three_chunks
 
     g = golden("3d_full_warp")
     it, k = 95, 32
     m = model_from_golden(g, probability_parameters=[float(g["pre_beta2"])], sparse_calculation_mode=True, sparse_top_k=k,
                           materialize_P=True)
-    _force_width(monkeypatch, m.NA, m.NB, m._cost_features(), _three_chunks(m.NB))
+    force_width(monkeypatch, m.NA, m.NB, m._cost_features(), three_chunks(m.NB))
     m.prepare()
     assert m.cost_plan.n_chunks == 3
     poke_golden_estep(m, g, it)
     m._params.cull = 1
-    emit = m._streamed_capture()
+    emit = m._capture_begin()
     chunks = []
 
     def grab(q, it_, c0, c1):

@@ -5,8 +5,6 @@ the device's dense P and the float64 oracle, in sparse mode, streamed in column 
 public interface (validation, SVI, the drivers, an unchanged run without it)."""
 
 import ctypes as C
-from concurrent.futures import ThreadPoolExecutor
-import threading
 
 import numpy as np
 import pytest
@@ -14,59 +12,13 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 from oracle import morpho_oracle as mo  # noqa: E402
+from layout_helpers import force_width, run_sharded, sharded_solvers, stream as _stream, three_chunks  # noqa: E402
 from parity_helpers import model_from_golden, poke_golden_estep  # noqa: E402
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # helpers
 # ---------------------------------------------------------------------------------------------------------------------
-def _stream():
-    import torch
-
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _force_width(monkeypatch, n_moving, n_fixed, features, width):
-    """Budget that fits a streamed run of ``width``-column chunks, and nothing wider."""
-    import torch
-
-    from spateo_release_b200.alignment import morpho_class as mc
-    from spateo_release_b200.alignment.distributed import pair_device_bytes
-
-    n_sms = torch.cuda.get_device_properties(0).multi_processor_count
-    budget = pair_device_bytes(n_moving, n_fixed, features, chunk_cols=width, n_sms=n_sms)
-    assert budget < pair_device_bytes(n_moving, n_fixed, features)
-    monkeypatch.setattr(mc, "_device_budget", lambda dev: budget)
-
-
-class _LockStep:
-    """Collectives of W shards of one process, each driven by its own thread, summed in rank order."""
-
-    def __init__(self, world):
-        self.bar = threading.Barrier(world, timeout=600)
-        self.slot = [None] * world
-
-    def _exchange(self, m, t):
-        self.slot[int(m.column_shard[0])] = t.clone()
-        self.bar.wait()
-        out = list(self.slot)
-        self.bar.wait()
-        return out
-
-    def sum_(self, m, view):
-        parts = self._exchange(m, view)
-        total = parts[0].clone()
-        for v in parts[1:]:
-            total += v
-        view.copy_(total)
-
-    def max_(self, m, keys):
-        keys.copy_(__import__("torch").stack(self._exchange(m, keys)).max(dim=0).values)
-
-    def gather(self, m, t):
-        return self._exchange(m, t)
-
-
 def _set_features(m, FB=None, FA=None):
     """Give a prepared solver transfer features (caller's row order) and their device buffers."""
     from spateo_release_b200 import _capi
@@ -293,16 +245,14 @@ def test_streamed_chunks_match_resident(monkeypatch):
     want = (want[0][:, :19], want[1])
 
     cols = res.NB
-    w = -(-(-(-cols // 3)) // 8) * 8
-    assert cols - 2 * w < w
-    _force_width(monkeypatch, res.NA, cols, res._cost_features(), w)
+    force_width(monkeypatch, res.NA, cols, res._cost_features(), three_chunks(cols))
     s = _pair_solver(A, B)
     s.prepare()
     assert s._streamed and s.cost_plan.n_chunks == 3
     poke_estep_state(s, *state)
     _set_features(s, FB, FA)
     st = _stream()
-    s._estep_only(25, st, on_chunk=s._streamed_capture())
+    s._estep_only(25, st, on_chunk=s._capture_begin())
     torch.cuda.synchronize()
     s._transfer_results(cols)
     assert np.array_equal(s.PT_FA, want[1])
@@ -313,8 +263,6 @@ def test_streamed_chunks_match_resident(monkeypatch):
 # 7. column-sharded pair (lock-step shards of one process)
 # ---------------------------------------------------------------------------------------------------------------------
 def _sharded_solvers(world, **opts):
-    import spateo_release_b200 as st
-    from spateo_release_b200.alignment.distributed import _HOST_INIT_FIELDS
     from spateo_release_b200.synthetic import make_slice_pair
 
     A, B = make_slice_pair(2600, 2300, 40, dim=3, seed=5, z_thickness=15.0, warp_amplitude=1.0)
@@ -324,44 +272,7 @@ def _sharded_solvers(world, **opts):
               transfer_B=np.concatenate([ones(A.shape[0]), rng.random((A.shape[0], 17))], axis=1).astype(np.float32),
               transfer_A=np.concatenate([ones(B.shape[0]), rng.random((B.shape[0], 2))], axis=1).astype(np.float32))
     kw.update(opts)
-    np.random.seed(0)
-    ref = st.align.Morpho_pairwise(sampleA=B, sampleB=A, **kw)
-    ref.prepare_host()
-    shards = []
-    for r in range(world):
-        np.random.seed(0)
-        m = st.align.Morpho_pairwise(sampleA=B, sampleB=A, column_shard=(r, world, "nccl"), **kw)
-        m.prepare_host()
-        shards.append(m)
-    for m in shards[1:]:
-        for k in _HOST_INIT_FIELDS:
-            if hasattr(shards[0], k):
-                setattr(m, k, getattr(shards[0], k))
-    for m in shards:
-        m.prepare_device()
-    return ref, shards
-
-
-def _run_sharded(shards):
-    import torch
-
-    st, m0 = _stream(), shards[0]
-    for it in range(m0.max_iter):
-        want_P = m0._captures_posterior and it == m0.max_iter - 1 and not (m0.return_mapping and m0.SVI_mode)
-        views = [m._shard_iteration_local(it, st, capture_P=want_P) for m in shards]
-        total = torch.zeros_like(views[0])
-        for v in views:
-            total += v
-        for v in views:
-            v.copy_(total)
-        for m in shards:
-            m._shard_iteration_finish(it, st)
-    comm = _LockStep(len(shards))
-    for m in shards:
-        m._shard_comm = comm
-    with ThreadPoolExecutor(len(shards)) as ex:
-        for f in [ex.submit(m._finish) for m in shards]:
-            f.result()
+    return sharded_solvers(A, B, world, **kw)
 
 
 @pytest.mark.parametrize("world", [2, 3])
@@ -369,7 +280,7 @@ def _run_sharded(shards):
 def test_column_sharded_transfer_matches_unsharded(world, opts):
     ref, shards = _sharded_solvers(world, **opts)
     ref.run()
-    _run_sharded(shards)
+    run_sharded(shards)
     m0 = shards[0]
     for m in shards:  # every replica holds the same bits
         assert np.array_equal(m.P_FB, m0.P_FB) and np.array_equal(m.PT_FA, m0.PT_FA)

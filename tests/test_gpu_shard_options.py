@@ -5,42 +5,13 @@ fold, ``_shard_iteration_finish`` after it) with the cross-rank sum of the row s
 closing ``_finish`` runs one thread per shard, whose collectives (``_shard_comm``) exchange through host memory."""
 
 import ctypes as C
-import threading
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
-
-class _LockStep:
-    """Collectives of W shards of one process, each driven by its own thread: sums in rank order, like the peer-memory
-    kernel, so every replica gets the same bits."""
-
-    def __init__(self, world):
-        self.bar = threading.Barrier(world, timeout=600)
-        self.slot = [None] * world
-
-    def _exchange(self, m, t):
-        self.slot[int(m.column_shard[0])] = t.clone()
-        self.bar.wait()
-        out = list(self.slot)
-        self.bar.wait()
-        return out
-
-    def sum_(self, m, view):
-        parts = self._exchange(m, view)
-        total = parts[0].clone()
-        for v in parts[1:]:
-            total += v
-        view.copy_(total)
-
-    def max_(self, m, keys):
-        keys.copy_(__import__("torch").stack(self._exchange(m, keys)).max(dim=0).values)
-
-    def gather(self, m, t):
-        return self._exchange(m, t)
+from layout_helpers import finish_all, run_sharded, sharded_solvers, stream as _stream  # noqa: E402
 
 
 def _pair():
@@ -57,67 +28,13 @@ def _guidance(A, B, n=24):
 
 def _solvers(world, **opts):
     """The unsharded solver and W shards with the same host initialisation (the driver broadcasts rank 0's)."""
-    import spateo_release_b200 as st
-    from spateo_release_b200.alignment.distributed import _HOST_INIT_FIELDS
-
     A, B = _pair()
     kw = dict(max_iter=110, K=15, nn_init=True, verbose=False, device="0", materialize_P=False)
     kw.update(opts)
     if kw.pop("guide", False):
         kw.update(guidance_pair=_guidance(A, B), guidance_effect="both")
-    np.random.seed(0)
-    ref = st.align.Morpho_pairwise(sampleA=B, sampleB=A, **kw)
-    ref.prepare_host()  # consumes the random stream (SVI batch permutation) before the shards reseed it
-    shards = []
-    for r in range(world):
-        np.random.seed(0)
-        m = st.align.Morpho_pairwise(sampleA=B, sampleB=A, column_shard=(r, world, "nccl"), **kw)
-        m.prepare_host()
-        shards.append(m)
-    for m in shards[1:]:
-        for k in _HOST_INIT_FIELDS:
-            if hasattr(shards[0], k):
-                setattr(m, k, getattr(shards[0], k))
-    for m in shards:
-        m.prepare_device()
+    ref, shards = sharded_solvers(A, B, world, **kw)
     return A, ref, shards
-
-
-def _stream():
-    import torch
-
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _lockstep_iterations(shards, iters):
-    import torch
-
-    st, m0 = _stream(), shards[0]
-    for it in iters:
-        want_P = ((m0.materialize_P or m0.compute_mapping) and it == m0.max_iter - 1
-                  and not (m0.return_mapping and m0.SVI_mode))
-        views = [m._shard_iteration_local(it, st, capture_P=want_P) for m in shards]
-        total = torch.zeros_like(views[0])
-        for v in views:  # rank order
-            total += v
-        for v in views:
-            v.copy_(total)
-        for m in shards:
-            m._shard_iteration_finish(it, st)
-
-
-def _finish_all(shards):
-    comm = _LockStep(len(shards))
-    for m in shards:
-        m._shard_comm = comm
-    with ThreadPoolExecutor(len(shards)) as ex:
-        for f in [ex.submit(m._finish) for m in shards]:
-            f.result()
-
-
-def _run_sharded(shards):
-    _lockstep_iterations(shards, range(shards[0].max_iter))
-    _finish_all(shards)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -136,7 +53,7 @@ _RUNS = {
 def test_sharded_run_matches_unsharded(world, case):
     A, ref, shards = _solvers(world, **_RUNS[case])
     ref.run()
-    _run_sharded(shards)
+    run_sharded(shards)
     scale = np.abs(ref.XAHat).max()
     for m in shards:
         assert np.abs(m.XAHat - ref.XAHat).max() < 2e-5 * scale
@@ -349,7 +266,7 @@ def test_sparse_posterior_whole_run(svi):
     k = 32
     A, ref, shards = _solvers(3, SVI_mode=svi, sparse_calculation_mode=True, sparse_top_k=k, materialize_P=True)
     P_ref = ref.run()
-    _run_sharded(shards)
+    run_sharded(shards)
     n_cols = ref.batch_size if svi else ref.NB
     top = np.abs(P_ref.data).max()
     for m in shards:
@@ -381,7 +298,7 @@ def test_mapping_from_identical_state(svi):
                                                C.c_void_p(rb.data_ptr()), C.c_void_p(cb.data_ptr()), st), "mapped")
     assert torch.equal(rb, ref._rowbest) and torch.equal(cb, ref._colbest)
     ref._finish()
-    _finish_all(shards)  # merges the row keys (maximum) and gathers the column keys
+    finish_all(shards)  # merges the row keys (maximum) and gathers the column keys
     Y = np.asarray(_pair()[0].obsm["spatial"])
     Y = Y[ref.batch_idx] if svi else Y
     want = st_.align.get_optimal_mapping_relationship(ref.optimal_RnA, Y, ref.mapping)

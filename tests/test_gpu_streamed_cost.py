@@ -8,28 +8,8 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 
+from layout_helpers import force_width as _force_width, three_chunks as _three_chunks  # noqa: E402
 from parity_helpers import cfg_of, model_from_golden, poke_golden_estep, relmax  # noqa: E402
-
-
-def _force_width(monkeypatch, n_moving, n_fixed, features, width):
-    """Budget that fits a streamed run of ``width``-column chunks, and nothing wider."""
-    import torch
-
-    from spateo_release_b200.alignment import morpho_class as mc
-    from spateo_release_b200.alignment.distributed import pair_device_bytes
-
-    n_sms = torch.cuda.get_device_properties(0).multi_processor_count
-    budget = pair_device_bytes(n_moving, n_fixed, features, chunk_cols=width, n_sms=n_sms)
-    assert budget < pair_device_bytes(n_moving, n_fixed, features)
-    monkeypatch.setattr(mc, "_device_budget", lambda dev: budget)
-
-
-def _three_chunks(cols):
-    """A width that splits ``cols`` columns into three chunks, the last one shorter."""
-    w = -(-cols // 3)
-    w = -(-w // 8) * 8
-    assert cols - 2 * w < w
-    return w
 
 
 def _pair(n=2600, nb=2400, genes=24, seed=2):

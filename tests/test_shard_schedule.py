@@ -10,8 +10,8 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from spateo_release_b200.alignment.distributed import all_gather_rows, assemble_columns, column_block
-from spateo_release_b200.alignment.morpho_class import Morpho_pairwise, shard_svi_schedule, svi_schedule
+from spateo_release_b200.alignment.distributed import Collectives, all_gather_rows, assemble_columns, column_block
+from spateo_release_b200.alignment.morpho_class import shard_svi_schedule, svi_schedule
 
 
 @pytest.mark.parametrize("world", [1, 2, 3, 7])
@@ -57,21 +57,19 @@ def test_assemble_columns_drops_null_and_gather_padding():
 
 
 def _worker(rank, world, port, q):
-    from types import SimpleNamespace
-
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
     dist.init_process_group("gloo", rank=rank, world_size=world)
-    # the solver's own collectives of a column-sharded pair (they touch no device state: a stand-in object will do)
-    shard = SimpleNamespace(_shard_mode="nccl")
+    # the solver's own collectives of a column-sharded pair (they touch no device state and ignore the solver)
+    comm = Collectives()
     rows = torch.arange(3 + 2 * rank, dtype=torch.int32).reshape(-1, 1) * 10 + rank  # 3 and 5 rows
-    parts = [p.numpy() for p in Morpho_pairwise._shard_gather(shard, rows)]
+    parts = [p.numpy() for p in comm.gather(None, rows)]
     # argmax keys: (float bits of p) << 32 | (0xffffffff - column); the row keys are merged with a MAX all_reduce
     vals = np.array([[0.5, 0.25, 0.0], [0.125, 0.75, 0.0]], dtype=np.float32)[rank]
     cols = np.array([[0, 1, 2], [3, 4, 5]], dtype=np.int64)[rank]
     keys = torch.from_numpy((vals.view(np.uint32).astype(np.int64) << 32) | (0xFFFFFFFF - cols))
-    Morpho_pairwise._shard_max_(shard, keys)
+    comm.max_(None, keys)
     view = torch.tensor([1.0, 2.0 ** -40, -3.0], dtype=torch.float64) * (rank + 1)  # row statistics of this rank
-    Morpho_pairwise._shard_sum(shard, view, None)
+    comm.sum_(None, view)
     q.put((rank, parts, keys.numpy(), view.numpy(), [p.numpy() for p in all_gather_rows(rows[:1])]))
     dist.destroy_process_group()
 
