@@ -12,5 +12,5 @@ from .morpho_class import Morpho_pairwise
 from .transform import BA_transform, field_eval
 from .utils import empty_cache, solve_RT_by_correspondence
 from .distributed import (align_chain_pipelined, column_block, gather_transformations, morpho_align_chain_sharded,
-                          morpho_align_pair_sharded, shard_pairs)
+                          morpho_align_column_sharded, morpho_align_pair_sharded, shard_pairs)
 from .mapping import ArgmaxPi, get_optimal_mapping_relationship, mapping_aligned_coords

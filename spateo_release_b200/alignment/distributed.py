@@ -4,18 +4,25 @@ transforms, then the serial prefix composition of the reference's ``morpho_align
 
 One process per GPU (``torchrun``); the data path has no collective — the pairs are independent problems — and the only
 exchange is ``[R(2x2) | t(2)]`` per pair (48 bytes), which is what BASELINE.json calls the global rigid-consensus step.
+
+Two more layouts split the work of ONE pair over the ranks instead: ``morpho_align_pair_sharded`` (one pair, its fixed
+cells column-sharded) and ``morpho_align_column_sharded`` (``morpho_align``'s serial chain, every pair column-sharded).
 """
 
 from __future__ import annotations
 
+import contextlib
 import gc
+import threading
 from typing import Callable, List, Optional
 
 import numpy as np
 import torch
 import torch.distributed as dist
 
-from .morpho_alignment import compose_transformations, pair_transformation
+from .morpho_alignment import (_seed_keys, _store_pair, _store_transfer, _transfer_keys, _working_copy,
+                               compose_transformations, pair_transformation)
+from .utils import empty_cache
 
 
 def shard_pairs(n_pairs: int, rank: int, world: int) -> List[int]:
@@ -62,7 +69,8 @@ def morpho_align_chain_sharded(
     **pairwise_kwargs,
 ):
     """Sharded equivalent of ``morpho_align_transformation`` + ``morpho_align_apply_transformation`` (rigid, 2-D, raw
-    coordinates — NOT bitwise ``morpho_align``, whose pairs are serially dependent; SURVEY.md §8(e)).
+    coordinates — NOT bitwise ``morpho_align``, whose pairs are serially dependent; SURVEY.md §8(e)). For ``morpho_align``'s
+    semantics over several GPUs see ``morpho_align_column_sharded``.
 
     Every rank receives the whole list of slices (or at least the ones it touches), aligns its pairs, joins the single
     all-gather, composes the chain and writes ``obsm[key_added]`` of every slice it holds. Returns
@@ -252,10 +260,11 @@ def column_block(n_cols: int, rank: int, world: int):
 
 
 class Collectives:
-    """The exchanges of a column-sharded pair's ranks, on ``torch.distributed``: in place sum and element-wise maximum, and
-    the gather of every rank's per-column rows in rank order. Without a process group of several ranks the sum and the
-    maximum leave ``t`` as it is and the gather returns this rank's own rows. ``m`` is the calling solver; tests that run
-    several shards in one process substitute an object with the same methods that tells the shards apart by it."""
+    """The exchanges of a column-sharded pair's ranks, on ``torch.distributed``: in place sum and element-wise maximum, the
+    gather of every rank's per-column rows in rank order, and the broadcast of rank 0's host objects. Without a process
+    group of several ranks the sum and the maximum leave ``t`` as it is, the gather returns this rank's own rows and the
+    broadcast returns ``obj``. ``m`` is the calling solver; tests that run several shards in one process substitute an
+    object with the same methods that tells the shards apart by it."""
 
     @staticmethod
     def _several_ranks() -> bool:
@@ -271,6 +280,14 @@ class Collectives:
 
     def gather(self, m, t: torch.Tensor) -> List[torch.Tensor]:
         return all_gather_rows(t) if self._several_ranks() else [t]
+
+    def broadcast(self, m, obj):
+        """Rank 0's ``obj`` (any picklable object; the other ranks pass None) on every rank."""
+        if not self._several_ranks():
+            return obj
+        box = [obj]
+        dist.broadcast_object_list(box, src=0)
+        return box[0]
 
 
 def assemble_columns(parts: List[np.ndarray], positions: List[np.ndarray], n_out: int, fill=0) -> np.ndarray:
@@ -315,8 +332,9 @@ def morpho_align_pair_sharded(fixed, moving, mode: str = "auto", device=None, **
     separate collective); ``mode="nccl"``: ``all_reduce`` + a finishing kernel (the baseline). The M-step runs replicated.
 
     Rank 0's inducing points and host initialisation (coarse rigid alignment, sigma2 / beta2 guesses, the SVI batch
-    permutation) are broadcast so the replicas start from the same bits whatever the ranks' NumPy random state. Returns the solver (same result attributes as ``Morpho_pairwise``; identical on
-    every rank).
+    permutation) are broadcast so the replicas start from the same bits whatever the ranks' NumPy random state; rank 0
+    draws them from the global ``np.random`` stream as ``Morpho_pairwise`` does, and every rank's stream ends where rank
+    0's does. Returns the solver (same result attributes as ``Morpho_pairwise``; identical on every rank).
 
     Runs the full EM unless the caller passes ``SVI_mode=True`` (earlier versions replaced an explicit ``SVI_mode=True``
     with the full EM without saying so). Under SVI every rank runs the members of each batch that fall in its block,
@@ -326,9 +344,6 @@ def morpho_align_pair_sharded(fixed, moving, mode: str = "auto", device=None, **
     unsharded column order. A dense ``materialize_P=True`` raises NotImplementedError, as does a pair whose block of the
     cost matrix does not fit its GPU. ``transfer_B`` / ``transfer_A`` take keys only, as in ``morpho_align``; after
     ``run()`` every rank holds the whole ``P_FB`` and ``PT_FA``."""
-    from .morpho_alignment import _transfer_keys
-    from .morpho_class import Morpho_pairwise
-
     _transfer_keys(pairwise_kwargs)
 
     world = dist.get_world_size() if dist.is_initialized() else 1
@@ -336,18 +351,124 @@ def morpho_align_pair_sharded(fixed, moving, mode: str = "auto", device=None, **
     kw = dict(pairwise_kwargs)
     kw.setdefault("materialize_P", False)
     kw.setdefault("SVI_mode", False)
-    solver = Morpho_pairwise(sampleA=moving, sampleB=fixed, device=device, column_shard=(rank, world, mode), **kw)
+    return _shard_solver(fixed, moving, rank, world, mode, device, Collectives(), **kw)
+
+
+# One lock per process around every shard's draws from the global NumPy stream: shards run by the threads of one process
+# (the tests emulate ranks that way) share that stream.
+_NP_STREAM = threading.Lock()
+
+
+@contextlib.contextmanager
+def _draws_of(rank: int):
+    """A shard's draws from the global ``np.random`` stream. Rank 0's are the unsharded solver's; another rank's are
+    replaced by rank 0's (broadcast), so it leaves the stream as it found it."""
+    with _NP_STREAM:
+        state = np.random.get_state() if rank else None
+        try:
+            yield
+        finally:
+            if state is not None:
+                np.random.set_state(state)
+
+
+def _shard_solver(fixed, moving, rank: int, world: int, exchange: str, device, comm, **kw):
+    """Shard ``rank`` of ``world`` of the pair, prepared for ``run()``, with ``comm`` (a ``Collectives``) for every
+    exchange: rank 0's inducing points and host initialisation broadcast to the others, whose NumPy stream then continues
+    from where rank 0's stands."""
+    from .morpho_class import Morpho_pairwise
+
+    with _draws_of(rank):
+        solver = Morpho_pairwise(sampleA=moving, sampleB=fixed, device=device, column_shard=(rank, world, exchange), **kw)
+    solver._shard_comm = comm
     if world > 1:  # rank 0's inducing points, so that every rank builds the same kernel matrices (U, Gamma, guidance U_I)
-        box = [solver.inducing_variables_idx if rank == 0 else None]
-        dist.broadcast_object_list(box, src=0)
-        if not np.array_equal(box[0], solver.inducing_variables_idx):
+        idx = comm.broadcast(solver, solver.inducing_variables_idx if rank == 0 else None)
+        if not np.array_equal(idx, solver.inducing_variables_idx):
             with torch.cuda.device(solver._dev):
-                solver._construct_kernel(box[0])
-    solver.prepare_host()
+                solver._construct_kernel(idx)
+    with _draws_of(rank):
+        solver.prepare_host()
+        stream = np.random.get_state() if rank == 0 else None
     if world > 1:
-        box = [{k: getattr(solver, k) for k in _HOST_INIT_FIELDS if hasattr(solver, k)} if rank == 0 else None]
-        dist.broadcast_object_list(box, src=0)
-        for k, v in box[0].items():
+        init = ({k: getattr(solver, k) for k in _HOST_INIT_FIELDS if hasattr(solver, k)}, stream) if rank == 0 else None
+        fields, stream = comm.broadcast(solver, init)
+        for k, v in fields.items():
             setattr(solver, k, v)
+        if rank:
+            with _NP_STREAM:
+                np.random.set_state(stream)
     solver.prepare_device()
     return solver
+
+
+def sharded_chain_pair(fixed, moving, pair: int, rank: int, world: int, comm, mode: str = "SN-S",
+                       exchange: str = "auto", device=None, **solver_kwargs):
+    """Pair ``pair`` of ``morpho_align_column_sharded`` on one rank: ``moving`` aligned onto ``fixed`` with this rank's
+    block of the fixed cells, every exchange through ``comm`` (a ``Collectives``), and the outputs written onto the two
+    slices as ``morpho_align`` writes them. ``solver_kwargs`` go to ``Morpho_pairwise`` (``spatial_key``, ``key_added``,
+    ``iter_key_added`` and ``vecfld_key_added`` among them). Returns the pair's entry of ``pis``: ``P.T``, or None when the
+    posterior is not materialised. The pair's device state (cost-matrix block, solver state, row-statistics buffer and its
+    symmetric-memory handle) is released before returning, so a chain holds one pair's at a time."""
+    try:
+        solver = _shard_solver(fixed, moving, rank, world, exchange, device, comm, **solver_kwargs)
+    except NotImplementedError as e:
+        if "column_shard" not in str(e):  # the refusal of a block that would have to be streamed (Morpho_pairwise._plan_cost)
+            raise
+        raise NotImplementedError(
+            f"pair {pair} (slice {pair + 1} onto slice {pair}), rank {rank} of {world}: {e}. More ranks would make each "
+            "rank's block of the cost matrix smaller, and resident") from e
+    P = solver.run()
+    _store_pair(moving, solver, solver.key_added, mode, solver.iter_key_added, solver.vecfld_key_added)
+    _store_transfer(fixed, moving, solver, *_transfer_keys(solver_kwargs))
+    # The last exchange of run() (the gather of K_NB) has completed on every rank, and with it every peer's reads of this
+    # rank's symmetric buffer, so the buffer can go.
+    del solver
+    gc.collect()
+    empty_cache()
+    return None if P is None else P.T
+
+
+def morpho_align_column_sharded(
+    models: List, rep_layer="X", rep_field="layer", genes=None, spatial_key: str = "spatial",
+    key_added: str = "align_spatial", iter_key_added: Optional[str] = "iter_spatial",
+    vecfld_key_added: str = "VecFld_morpho", mode: str = "SN-S", dissimilarity="kl", max_iter: int = 200,
+    dtype: str = "float32", device=None, verbose: bool = True, exchange: str = "auto", **kwargs,
+):
+    """``morpho_align`` with every slice pair column-sharded over the ranks of the process group (one process per GPU,
+    ``torchrun``; without a process group it runs on one GPU). Same signature, defaults, pairs, order and ``.obsm`` /
+    ``.uns`` keys as ``morpho_align``: pair i aligns slice i+1 onto slice i's aligned coordinates (``key_added``), SN-S /
+    SN-N, 2-D or 3-D, the non-rigid field stored per slice; inputs are not mutated. Returns ``(align_models, pis)``.
+
+    Every pair runs through ``morpho_align_pair_sharded``'s solver: each rank holds 1/W of the pair's cost matrix, so pairs
+    stay resident on their GPUs up to about sqrt(W) times the slice size one GPU holds. ``exchange``: how the ranks sum the
+    per-row statistics ("auto", "p2p" or "nccl", the ``mode`` of ``morpho_align_pair_sharded``).
+
+    ``np.random.seed(s)`` on rank 0 before the call gives rank 0 the draws ``morpho_align`` makes after the same seed,
+    pair by pair (inducing points, coarse initialisation, SVI batch permutation); the other ranks use rank 0's, and every
+    rank's stream ends where rank 0's does. Every rank returns the same slices.
+
+    Defaults that differ from ``morpho_align_pair_sharded``'s: ``SVI_mode=True`` (the reference's) and
+    ``materialize_P=False``. ``pis[i]`` is the gathered ``scipy.sparse.coo_matrix`` ``P.T`` with
+    ``sparse_calculation_mode=True, materialize_P=True``, otherwise None; a dense ``materialize_P`` raises
+    NotImplementedError, as does a pair whose block of the cost matrix does not fit its GPU (a sharded block is not
+    streamed). ``transfer_B`` / ``transfer_A``: keys only, as in ``morpho_align``."""
+    kwargs.setdefault("SVI_mode", True)
+    kwargs.setdefault("materialize_P", False)
+    if kwargs["materialize_P"] and not kwargs.get("sparse_calculation_mode", False):
+        raise NotImplementedError("materialize_P (dense) on column-sharded pairs: the N_A x N_B posterior does not fit "
+                                  "one GPU; pass sparse_calculation_mode=True for the sparse posterior")
+    _transfer_keys(kwargs)
+    world = dist.get_world_size() if dist.is_initialized() else 1
+    rank = dist.get_rank() if dist.is_initialized() else 0
+    comm = Collectives()
+    aligned = [_working_copy(m) for m in models]
+    _seed_keys(aligned, spatial_key, key_added)
+    pis = []
+    for i, (fixed, moving) in enumerate(zip(aligned[:-1], aligned[1:])):
+        pis.append(sharded_chain_pair(
+            fixed, moving, i, rank, world, comm, mode=mode, exchange=exchange, device=device, rep_layer=rep_layer,
+            rep_field=rep_field, dissimilarity=dissimilarity, genes=genes, spatial_key=key_added, key_added=key_added,
+            iter_key_added=iter_key_added, vecfld_key_added=vecfld_key_added, max_iter=max_iter, dtype=dtype,
+            verbose=verbose and rank == 0, **kwargs,
+        ))
+    return aligned, pis

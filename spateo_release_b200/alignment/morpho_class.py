@@ -383,7 +383,8 @@ class Morpho_pairwise:
     (SPB_ROW_TILE = 512 cells) and each of its four 128-cell quarters is spatially compact, and the (quarter, fixed cell) pairs
     of rows whose every pair underflows to exactly 0 in fp32 are neither read nor computed; results are bit-identical to the
     dense sweep in the same row order (all outputs are returned in the caller's row order).
-    ``column_shard`` — set by ``morpho_align_pair_sharded``: one pair's fixed cells split over several GPUs. A shard runs
+    ``column_shard`` — set by ``morpho_align_pair_sharded`` and ``morpho_align_column_sharded``: one pair's fixed cells
+    split over several GPUs. A shard runs
     the full EM or SVI (each rank runs its members of every batch, padded with a null column), with ``return_mapping``,
     guidance, ``sparse_calculation_mode`` and ``compute_mapping``; ``K_NB``, ``P`` (sparse COO) and ``mapping`` are gathered
     into the unsharded column order on every rank. A dense ``materialize_P=True`` is refused (NotImplementedError).
@@ -403,8 +404,7 @@ class Morpho_pairwise:
     ``return_mapping=True``, whose closing E-step covers every fixed cell. Resident, streamed and column-sharded pairs.
     Accepted but without effect (memory work-arounds whose results are identical): ``use_chunk``, ``chunk_capacity``,
     ``pre_compute_dist``. ``sparse_calculation_mode`` keeps the top ``sparse_top_k`` posterior entries of every column by an
-    exact on-device radix select (P comes back as ``scipy.sparse.coo_matrix``). Not implemented (NotImplementedError):
-    ``kernel_type="geodist"``.
+    exact on-device radix select (P comes back as ``scipy.sparse.coo_matrix``).
     """
 
     def __init__(
